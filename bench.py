@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- leapfrog-steps/sec (all chains) of the B200-native HMC hot path, with the HBM
+"""bench.py -- leapfrog-steps/sec (all chains) of the H100-native HMC hot path, with the HBM
 roofline of the vectorised leapfrog kernel and the CPU baseline timed beside it.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (torchrun launches N>1)
@@ -75,7 +75,7 @@ def dense_matrices(D):
 
 
 # ------------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md "clocks DURING the timed region")
+# clocks sampled DURING the timed region
 # ------------------------------------------------------------------------------------------------------
 class ClockSampler:
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -327,16 +327,30 @@ def load_peaks():
         return {}
 
 
-def ncu_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of a kernel at its benchmark shape, from the committed
-    `ncu --set full` capture summaries (profiles/r02_traffic.json, written by scripts/ncu_traffic.py from the .ncu-rep of the
-    same command); None when no capture of that kernel is committed."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        e = t.get(kernel_key)
-        return (float(e["dram_bytes"]), e["source"]) if e else (None, None)
-    except Exception:
-        return None, None
+# Fallback peaks when no measured figure is given: NVIDIA's H100 SXM data sheet (700 W card), never reached in practice
+DATASHEET_HBM_GBS = 3350.0
+DATASHEET_FP16_TFLOPS = 989.0
+DUMP_BYTES = 64_000_000
+
+
+def dump_outputs(out_dir, arrays, n_rows):
+    """Write what the timed path returned in its last step as out_dir/<name>.npy (float32, float64 for the chain index).
+    Arrays with one row per chain are cut to a fixed, seeded sample of chains so that the dump stays under 64 MB; the
+    sampled chain indices are written as chain_index.npy."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    host = {k: torch.as_tensor(v).detach().float().cpu().numpy() for k, v in arrays.items()}
+    per_row = 8 + sum(a.nbytes // n_rows for a in host.values() if a.shape[:1] == (n_rows,))   # + the chain index
+    other = sum(a.nbytes for a in host.values() if a.shape[:1] != (n_rows,))
+    budget = DUMP_BYTES - 100_000   # headroom for the .npy headers
+    rows = np.arange(n_rows)
+    if other + per_row * n_rows > budget:
+        keep = max(1, (budget - other) // per_row)
+        rows = np.sort(np.random.default_rng(0).choice(n_rows, size=min(keep, n_rows), replace=False))
+    for k, a in host.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a[rows] if a.shape[:1] == (n_rows,) else a)
+    np.save(os.path.join(out_dir, "chain_index.npy"), rows.astype(np.float64))
 
 
 def run_nuts_workload(args, wl, dev, dist, world, rank, local_rank):
@@ -408,6 +422,16 @@ def run_nuts_workload(args, wl, dev, dist, world, rank, local_rank):
     barrier()
     ms_total = e0.elapsed_time(e1)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        if adapt:
+            st, params = out
+            arrays = {"step_size": params["step_size"], "inverse_mass_matrix": params["inverse_mass_matrix"]}
+        else:
+            st = out[0]
+            arrays = {"acceptance_rate": out[1]} if BLK > 1 else {
+                "acceptance_rate": out[1].acceptance_rate, "num_integration_steps": out[1].num_integration_steps}
+        arrays.update(position=st.position, logdensity=st.logdensity, logdensity_grad=st.logdensity_grad)
+        dump_outputs(args.dump_outputs, arrays, C)
     if dist is not None:
         allc = [None] * world
         dist.all_gather_object(allc, clocks)
@@ -466,7 +490,7 @@ def run_nuts_workload(args, wl, dev, dist, world, rank, local_rank):
     if rank != 0:
         return
     peaks = load_peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", DATASHEET_HBM_GBS))
     value = n_lf / (ms_total * 1e-3)
     transitions = K * (T if adapt else BLK)
     # The HBM roofline of the path is that of the vectorised one-step leapfrog kernel (24*D bytes per chain per launch,
@@ -493,7 +517,6 @@ def run_nuts_workload(args, wl, dev, dist, world, rank, local_rank):
     ms_1step = f0.elapsed_time(f1) / n1
     achieved = 24.0 * C * D / (ms_1step * 1e-3) / 1e9
     del q1, p1, g1, deng
-    traffic, traffic_src = ncu_traffic(f"k_leapfrog_diag_{C}x{D}")
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": n_gpus, "steps": K, "warmup": W,
         "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -510,15 +533,15 @@ def run_nuts_workload(args, wl, dev, dist, world, rank, local_rank):
                    "l2": "state arrays %.0f MB per GPU (workspace rows 9 + 2*depth); inputs exceed L2" % (C * D * 4 / 1e6),
                    "mean_tree_size": n_lf / (n_gpus * C * transitions), "ms_per_transition": ms_total / transitions},
         "roofline": {"bound": "hbm", "kernel": "k_leapfrog (diag metric, 1 step/launch, 24*D B per chain) at this workload's chains x dims",
-                     "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                     "traffic_source": traffic_src, "avg_launch_ms": ms_1step, "launches_timed": n1,
-                     "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"},
+                     "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+                     "avg_launch_ms": ms_1step, "launches_timed": n1,
+                     "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks
+                     else "H100 SXM data sheet, 3350 GB/s"},
         "tree_kernel": {"kernel": "k_nuts_doubling (one launch for doublings 0-3 over all chains, then one per further doubling over "
                         "the compacted list; row counts stay on the device: no host round trip)" if (adapt or BLK == 1) else
                         "k_nuts_chains (persistent grid; every warp takes whole chains through all transitions of the call)",
                         "equivalent_GBps_at_24D_per_leapfrog": 24.0 * D * value / n_gpus / 1e9,
-                        "bound": "dependent-instruction latency / issue slots (rows are register-resident inside a launch); "
-                                 "ncu issue-slot figures: profiles/r02_ncu_nuts.md"},
+                        "bound": "dependent-instruction latency / issue slots (rows are register-resident inside a launch)"},
         "e2e": {"value": n_lf_e2e / (ms_e2e * 1e-3), "unit": UNIT, "h2d_bytes_per_step": C * D * 4 + 8,
                 "d2h_bytes_per_step": C * D * 4 + C * 4, "steps": K_e2e, "ms_per_step": ms_e2e / K_e2e},
         "gpu_launches": K * ((T * 7 + 2) if adapt else (4 if BLK == 1 else 3)),
@@ -544,6 +567,8 @@ def main():
     ap.add_argument("--workload", default=DEFAULT_WORKLOAD, choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--e2e-chunks", type=int, default=4, help="chain slices (streams) of the end-to-end leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (a fixed chain sample, <= 64 MB)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     wl = WORKLOADS[args.workload]
@@ -629,6 +654,10 @@ def main():
     launches = K * (1 if not dense else (4 * L + 10))
     acc_mean = float(info.acceptance_rate.mean())
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"position": state.position, "logdensity": state.logdensity,
+                                         "logdensity_grad": state.logdensity_grad, "acceptance_rate": info.acceptance_rate,
+                                         "is_accepted": info.is_accepted}, C)
     if dist is not None:  # rank 0 reports the slowest GPU's median SM clock and the union of throttle reasons
         all_clocks = [None] * world
         dist.all_gather_object(all_clocks, clocks)
@@ -741,32 +770,28 @@ def main():
 
     if rank == 0:
         peaks = load_peaks()
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        peak = float(peaks.get("hbm_gbs", DATASHEET_HBM_GBS))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         bytes_1step = 24.0 * C * D
         achieved = bytes_1step / (ms_1step * 1e-3) / 1e9
         ms_step = ms_total / K
-        traffic_leapfrog, src_leapfrog = ncu_traffic("k_leapfrog_diag_65536x1024") if (C, D) == (65536, 1024) else (None, None)
-        traffic_gemm, src_gemm = ncu_traffic("k_gemm_f16x3_fused_65536x1024") if (C, D) == (65536, 1024) else (None, None)
         hbm_roofline = {"bound": "hbm", "kernel": "k_leapfrog (diag metric, 1 step/launch, 24*D B per chain)",
                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                        "traffic": traffic_leapfrog, "traffic_source": src_leapfrog,
                         "peak_source": peak_src, "avg_launch_ms": ms_1step, "launches_timed": n1}
         if dense:
-            burst = float(peaks.get("bf16_tflops", 1590.0))
-            tpeak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+            burst = float(peaks.get("bf16_tflops", DATASHEET_FP16_TFLOPS))
+            tpeak = float(peaks.get("bf16_tflops_sustained", DATASHEET_FP16_TFLOPS))
             tf_achieved = 2.0 * C * D * D / (ms_gemm * 1e-3) / 1e12
             roofline = {"bound": "tensor",
-                        "kernel": "bjx::k_gemm_f16x3, fused form (hand-written tcgen05.mma.cta_group::2 + TMA; epilogue: Cin, per-row "
+                        "kernel": "bjx::k_gemm_f16x3, fused form (hand-written wgmma + TMA; epilogue: Cin, per-row "
                                   "lincomb / double kick, Y, operand planes of Y for the next product); float32-accurate: 3 fp16 "
                                   "products per float32 product (ceiling frac = 1/3)",
                         "achieved": tf_achieved, "peak": tpeak, "unit": "TFLOP/s", "frac": tf_achieved / tpeak,
                         "frac_of_burst_peak": tf_achieved / burst, "burst_peak": burst,
-                        "traffic": traffic_gemm, "traffic_source": src_gemm,
                         "algorithmic_bytes": 16.0 * C * D,
                         "peak_source": ("measured sustained bf16 (MEASURED_PEAKS.json bf16_tflops_sustained): the kernel is timed inside "
                                         "a run of leapfrog steps under the power cap" if "bf16_tflops_sustained" in peaks
-                                        else "fallback 1400 TFLOP/s sustained"),
+                                        else "H100 SXM data sheet, 989 TFLOP/s dense FP16"),
                         "avg_launch_ms": ms_gemm, "launches_timed": n_prod,
                         "note": "algorithmic float32 flops 2*C*D^2 per launch; CUDA events on the engine's stream around 2 x 20 "
                                 "leapfrog steps = 80 products, row kernels and window checks of those steps charged to the products",
@@ -781,11 +806,13 @@ def main():
                                           "speedup_vs_1step_launches": (ms_1step * L) / ms_step}}
             if hier:  # the transition kernel is bound by the model's transcendental work, not by HBM: report it beside
                 n_obs = 8.0 * (D - 4)
+                n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+                sm_max_hz = (clocks.get("sm_max_mhz") or 1980.0) * 1e6   # H100 SXM's maximum SM clock when not sampled
                 mufu = (2.0 * (L - 1) + 3.0) * n_obs * C  # ex2 + rcp per observation; + lg2 where the log-density is live
                 extra["model_compute"] = {"sigmoid_evals_per_s": n_obs * C * L / (ms_step * 1e-3),
                                           "mufu_per_s": mufu / (ms_step * 1e-3),
-                                          "mufu_peak_per_s": 148 * 16 * 1.965e9,
-                                          "note": "16 MUFU lanes/clk/SM x 148 SMs at the maximum SM clock"}
+                                          "mufu_peak_per_s": n_sms * 16 * sm_max_hz,
+                                          "note": f"16 MUFU lanes/clk/SM x {n_sms} SMs at the maximum SM clock"}
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": n_gpus, "steps": K, "warmup": W,
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,

@@ -1,9 +1,9 @@
-"""blackjax_b200 -- B200-native HMC/NUTS hot path behind BlackJAX's API.
+"""blackjax_b200 -- H100-native HMC/NUTS hot path behind BlackJAX's API.
 
 ``import blackjax_b200 as blackjax`` gives ``blackjax.hmc``, ``blackjax.nuts`` and
 ``blackjax.window_adaptation`` with the reference's ``init / build_kernel / __call__ ->
 SamplingAlgorithm(init, step)`` surface (blackjax/__init__.py:70-80,104-112), natively batched over
-chains and executed by hand-written sm_100a CUDA kernels through the C ABI in ``include/bjx.h``.
+chains and executed by hand-written sm_90a CUDA kernels through the C ABI in ``include/bjx.h``.
 """
 import functools as _functools
 

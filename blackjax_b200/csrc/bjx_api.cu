@@ -908,9 +908,7 @@ extern "C" int bjx_nuts_sample(bjx_handle_t h, const uint32_t* rng_key, float* q
       a.sample.nint_history = num_integration_steps_history;
       a.sample.leapfrogs = nullptr;
       a.sample.queue = h->ws.counters + 62;
-      int sms = 148;
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->cfg.device);
-      a.grid_override = sms;  // the launcher multiplies by the CTAs that stay resident per SM
+      a.grid_override = sm_count();  // the launcher multiplies by the CTAs that stay resident per SM
       rc = dispatch(h, K_NUTS_CHAINS, true, a);
       h->last_leaf_launches = 1;
       h->last_depth = -1;
@@ -976,7 +974,7 @@ extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_r
              ? bjx_nuts_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, max_num_doublings, &info, nullptr, nullptr)
              : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, num_integration_steps, &info);
     if (rc == 0 && info.num_integration_steps) {  // executed leapfrogs, accumulated on the device (bench.py)
-      k_accum_steps<<<148, 256, 0, h->stream>>>(h->cfg.n_chains, steps_scratch, leapfrog_counter);
+      k_accum_steps<<<sm_count(), 256, 0, h->stream>>>(h->cfg.n_chains, steps_scratch, leapfrog_counter);
       BJX_CHECK_LAUNCH("k_accum_steps");
     }
     if (rc == 0)

@@ -404,7 +404,7 @@ static int dense_ws(bjx_handle_t h, DenseWs& w) {
   for (int m = 0; m < 3; ++m) {
     if (src[m] && (h->dense_mat_src[m] != src[m] || h->dense_mat_ver[m] != h->dense_version)) {
       DN_CUDA(cudaMemsetAsync(w.mat_max + m, 0, sizeof(float), h->stream));
-      k_absmax<<<148, 256, 0, h->stream>>>((long long)D * D / 4, src[m], w.mat_max + m);
+      k_absmax<<<sm_count(), 256, 0, h->stream>>>((long long)D * D / 4, src[m], w.mat_max + m);
       DN_LAUNCH("k_absmax");
       k_matrix_split2<<<g4((long long)D * D / 4), 256, 0, h->stream>>>((long long)D, (int)D, src[m], h->dense_mat_s[m],
                                                                       w.mat_max + m, w.mat_unscale + m);
@@ -475,7 +475,6 @@ static int gemm(bjx_handle_t h, DenseWs& w, const Part& pt, const float* X, int 
   g.epi.has_cin = Cin ? 1 : 0;
   g.epi.double_kick = double_kick ? 1 : 0;
   g.epi.planes = 0;
-  g.epi.debug = 0;
   g.epi.out_unscale = nullptr; g.epi.stale_max = nullptr; g.epi.next_max = nullptr; g.epi.zero_max = nullptr;
   if (po.var >= 0) {
     float* ring = w.rmax[po.var];

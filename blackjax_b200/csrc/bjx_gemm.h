@@ -42,7 +42,6 @@ struct GemmEpilogue {
   const float* stale_max;      // [M] row maxima of the previous production of this variable (chooses the lift)
   float* next_max;             // [M] this production's row maxima (atomic max; zero on entry)
   float* zero_max;             // [M] cleared for the production after this one
-  int debug;                   // timing experiments only (BJX_GEMM_DEBUG): 1 no Cin loads, 2 no plane stores, 4 no Y stores, 8 no math
 };
 
 struct GemmCall {

@@ -4,6 +4,13 @@
 #include <stdint.h>
 
 namespace bjx {
+// SMs of the current device: sizes the fixed grids of the grid-stride kernels
+inline int sm_count() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms > 0 ? sms : 1;
+}
 void launch_prng_split(const uint32_t* keys, long long n, int num, uint32_t* out, cudaStream_t s);
 void launch_prng_fold_in(const uint32_t* keys, long long n, uint32_t data, uint32_t* out, cudaStream_t s);
 void launch_prng_draw(int mode, const uint32_t* keys, long long n, long long per_key, void* out, cudaStream_t s);

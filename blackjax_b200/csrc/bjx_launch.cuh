@@ -4,6 +4,7 @@
 #pragma once
 #include <algorithm>
 
+#include "bjx_internal.h"
 #include "bjx_kernels.cuh"
 
 namespace bjx {
@@ -75,7 +76,7 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
   const int n_rows = (kernel_id == K_NUTS_DOUBLING) ? a.n_in : a.P.C;
   dim3 grid((n_rows + kWarpsPerBlock - 1) / kWarpsPerBlock), block(kThreads);
   // row count only known on the device: a fixed grid of 6 CTAs per SM strides over the compacted list
-  if (kernel_id == K_NUTS_DOUBLING && a.n_in_dev && grid.x > 148u * 6u) grid.x = 148u * 6u;
+  if (kernel_id == K_NUTS_DOUBLING && a.n_in_dev) grid.x = std::min(grid.x, 6u * (unsigned)sm_count());
   size_t smem = needs_row_smem<TK, DM>() ? sizeof(float) * kWarpsPerBlock * a.P.D : 0;
   if (kernel_id == K_NUTS_DOUBLING && a.ckpt_smem) smem += sizeof(float) * kWarpsPerBlock * 2 * a.depth_end * a.P.D;
   cudaStream_t st = a.stream;

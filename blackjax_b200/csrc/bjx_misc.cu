@@ -530,7 +530,7 @@ void launch_ess(int T, int C, int D, const float* hist, float* ess, float* scrat
   const int lag_blocks = (T + kEssLags - 1) / kEssLags;
   // enough chain chunks to fill the GPU, few enough that the double atomics stay rare
   const int d_blocks = (D + 31) / 32;
-  int chunks = (4 * 148 + d_blocks * lag_blocks - 1) / (d_blocks * lag_blocks);
+  int chunks = (4 * sm_count() + d_blocks * lag_blocks - 1) / (d_blocks * lag_blocks);
   chunks = chunks < 1 ? 1 : chunks;
   const int max_chunks = (C + kEssWarps - 1) / kEssWarps;
   chunks = chunks > max_chunks ? max_chunks : chunks;

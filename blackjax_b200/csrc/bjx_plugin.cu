@@ -1,7 +1,7 @@
 // Translation unit of a user-defined target plug-in (include/bjx_user_target.h, bjx_plugin_load in include/bjx.h).
 // Built once per target by blackjax_b200/plugin.py (or by hand):
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -Xcompiler -fPIC -shared \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Xcompiler -fPIC -shared \
 //        -I blackjax_b200/csrc -I include -DBJX_USER_SOURCE='"my_target.cuh"' [-DBJX_BUILD_SC=<size class>] \
 //        blackjax_b200/csrc/bjx_plugin.cu -o libbjxt_my_target.so
 //

@@ -72,31 +72,21 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-// ---- Blackwell packed FP32 (FFMA2 / FMUL2 / FADD2): two IEEE round-to-nearest operations per issue slot ----
-// sm_100 adds fma/mul/add.rn.f32x2 on 64-bit register pairs.  The leapfrog inner loop is FP32-issue bound
-// once the chain row lives in registers, so every elementwise update below goes through these helpers
-// (pairs of adjacent slots; odd slot counts fall back to scalar ops).  Results are bit-identical to the
-// scalar fmaf / * / + they replace.
+// ---- paired elementwise FP32 ops: explicit IEEE round-to-nearest, never contracted ----
+// Every elementwise update below goes through these helpers on pairs of adjacent slots (odd slot counts use
+// plain scalar ops), with the dot products keeping two interleaved accumulators.  The _rn intrinsics stop the
+// compiler from fusing a product into a later add, so each result is the one rounded operation written here.
 __device__ __forceinline__ void fma2(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-  asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\t"
-      "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
+  d0 = __fmaf_rn(a0, b0, c0);
+  d1 = __fmaf_rn(a1, b1, c1);
 }
 __device__ __forceinline__ void mul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\t"
-      "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-      "mul.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fmul_rn(a0, b0);
+  d1 = __fmul_rn(a1, b1);
 }
 __device__ __forceinline__ void add2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\t"
-      "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-      "add.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fadd_rn(a0, b0);
+  d1 = __fadd_rn(a1, b1);
 }
 
 // ---- user-defined targets (TK_USER; include/bjx_user_target.h) -----------------------------------------------------

@@ -1,6 +1,6 @@
 """NUTS behind BlackJAX's surface (blackjax/mcmc/nuts.py): iterative tree doubling driven from host
 C++ (libbjx ``bjx_nuts_step``), every leapfrog leaf and the per-chain energy / U-turn reductions as
-sm_100a kernels.  See :mod:`blackjax_b200.mcmc.hmc` for the batched-surface conventions."""
+sm_90a kernels.  See :mod:`blackjax_b200.mcmc.hmc` for the batched-surface conventions."""
 from typing import NamedTuple, Optional
 
 import torch

@@ -92,7 +92,7 @@ def build_plugin(source, dim, name="user", dense_metric=True, general_integrator
     with open(src, "w") as f:
         f.write(source)
     tmp = path + f".tmp{os.getpid()}"
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
            "-shared", "-I", CSRC, "-I", INCLUDE, f"-DBJX_USER_SOURCE=\"{src}\""]
     if sc == SC_BIG:
         cmd += ["-DBJX_PLUGIN_BIG=1"]

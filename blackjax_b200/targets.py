@@ -2,7 +2,7 @@
 
 BlackJAX accepts any JAX callable as ``logdensity_fn`` and differentiates it with
 ``jax.value_and_grad`` (blackjax/mcmc/hmc.py:91, integrators.py:189).  Without a tracing compiler the
-B200 path takes a *target descriptor* in the ``logdensity_fn`` slot instead: one of the named models
+H100 path takes a *target descriptor* in the ``logdensity_fn`` slot instead: one of the named models
 below, each with a hand-derived gradient fused into the leapfrog kernels
 (blackjax_b200/csrc/bjx_row.cuh ``Ctx::value_and_grad``), or a ``UserTarget``: the user's own fused
 ``value_and_grad`` as CUDA source, compiled into a plug-in that holds every kernel of the path

@@ -1,5 +1,5 @@
 /*
- * bjx.h -- C ABI of the B200-native HMC/NUTS hot path (libbjx.so).
+ * bjx.h -- C ABI of the H100-native HMC/NUTS hot path (libbjx.so).
  *
  * Drop-in boundary for BlackJAX's `blackjax.hmc` / `blackjax.nuts` / `window_adaptation`
  * path (reference: blackjax-devs/blackjax @ 63912a4).  The reference has no FFI of its own

