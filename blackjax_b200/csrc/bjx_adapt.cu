@@ -217,17 +217,6 @@ static NcclApi& nccl() {
 
 using namespace bjx;
 
-#define AD_CUDA(call)                                                \
-  do {                                                               \
-    cudaError_t e_ = (call);                                         \
-    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, #call);       \
-  } while (0)
-#define AD_LAUNCH(where)                                             \
-  do {                                                               \
-    cudaError_t e_ = cudaGetLastError();                             \
-    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, where);       \
-  } while (0)
-
 static int nccl_fail(bjx_handle_t h, ncclResult_t r, const char* where) {
   NcclApi& a = nccl();
   return bjx_fail(h, BJX_E_UNSUPPORTED, std::string(where) + ": " + (a.GetErrorString ? a.GetErrorString(r) : "NCCL error"));
@@ -266,9 +255,9 @@ extern "C" int bjx_nccl_comm_destroy(void* comm) {
 
 extern "C" int bjx_allgather_stats(bjx_handle_t h, void* nccl_comm, const float* block, int64_t count, float* gathered) {
   if (!h || !block || !gathered || count <= 0) return bjx_fail(h, BJX_E_INVALID, "bad argument");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (!nccl_comm) {  // one rank: the gathered array is the block
-    if (gathered != block) AD_CUDA(cudaMemcpyAsync(gathered, block, (size_t)count * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+    if (gathered != block) BJX_CUDA(cudaMemcpyAsync(gathered, block, (size_t)count * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
     return 0;
   }
   NcclApi& a = nccl();
@@ -288,12 +277,12 @@ extern "C" int64_t bjx_adapt_shared_state_floats(int32_t n_chains_local, int32_t
 extern "C" int bjx_adapt_shared_init(bjx_handle_t h, float* state, float initial_step_size, float* step_size_chain_out, float* imm_out) {
   if (!h || !state || !step_size_chain_out || !imm_out) return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (!(initial_step_size > 0.f)) return bjx_fail(h, BJX_E_INVALID, "initial_step_size must be positive");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   k_adapt_init<<<1, 256, 0, h->stream>>>(D, state, initial_step_size, imm_out);
-  AD_LAUNCH("k_adapt_init");
+  BJX_CHECK_LAUNCH("k_adapt_init");
   k_fill_from<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + 5, step_size_chain_out);
-  AD_LAUNCH("k_fill_from");
+  BJX_CHECK_LAUNCH("k_fill_from");
   return bjx_set_metric(h, BJX_METRIC_DIAG, imm_out);
 }
 
@@ -303,14 +292,14 @@ extern "C" int bjx_adapt_shared_update(bjx_handle_t h, void* nccl_comm, int32_t 
   if (!h || !state || !q || !acceptance_rate || !step_size_chain || !imm) return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
   if (window_end && stage != 1) return bjx_fail(h, BJX_E_INVALID, "a window ends on a slow-stage step");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   const int nb = n_stat_blocks(C);
   const size_t blk = 2 + 2 * (size_t)D;
   float* local = state + kHdr + 2 * (size_t)D;
   float* gathered = local + (size_t)nb * blk;
   k_block_stats<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, h->stream>>>(C, D, q, acceptance_rate, local);
-  AD_LAUNCH("k_block_stats");
+  BJX_CHECK_LAUNCH("k_block_stats");
   const float* merged_in = local;
   if (n_ranks > 1) {
     int rc = bjx_allgather_stats(h, nccl_comm, local, (int64_t)(nb * blk), gathered);
@@ -318,18 +307,18 @@ extern "C" int bjx_adapt_shared_update(bjx_handle_t h, void* nccl_comm, int32_t 
     merged_in = gathered;
   }
   k_shared_adapt<<<1, 512, 0, h->stream>>>(D, nb * n_ranks, merged_in, state, stage, window_end, target_acceptance, imm, eps_history);
-  AD_LAUNCH("k_shared_adapt");
+  BJX_CHECK_LAUNCH("k_shared_adapt");
   k_fill_from<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + 5, step_size_chain);
-  AD_LAUNCH("k_fill_from");
+  BJX_CHECK_LAUNCH("k_fill_from");
   if (window_end) return bjx_set_metric(h, BJX_METRIC_DIAG, imm);  // mass_matrix_sqrt of the new metric, on the stream
   return 0;
 }
 
 extern "C" int bjx_adapt_shared_final(bjx_handle_t h, const float* state, float* step_size_out) {
   if (!h || !state || !step_size_out) return bjx_fail(h, BJX_E_INVALID, "null argument");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_da(3, 1, const_cast<float*>(state), nullptr, 0.f, step_size_out, h->stream);  // exp(log_step_avg)
-  AD_LAUNCH("k_da_final");
+  BJX_CHECK_LAUNCH("k_da_final");
   return 0;
 }
 
@@ -570,13 +559,13 @@ extern "C" int bjx_chees_init(bjx_handle_t h, float* state, float step_size, int
                               float* step_size_chain_out, int32_t* steps_chain_out) {
   if (!h || !state || !step_size_chain_out || !steps_chain_out) return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (!(step_size > 0.f) || max_bits < 1 || max_bits > 30) return bjx_fail(h, BJX_E_INVALID, "bad step_size / max_bits");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int C = h->cfg.n_chains;
   k_chees_init<<<1, 32, 0, h->stream>>>(state, step_size, max_bits, jitter_amount);
-  AD_LAUNCH("k_chees_init");
+  BJX_CHECK_LAUNCH("k_chees_init");
   k_fill_from<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + CH_EPS, step_size_chain_out);
   k_fill_steps<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + CH_L, steps_chain_out);
-  AD_LAUNCH("k_fill");
+  BJX_CHECK_LAUNCH("k_fill");
   return 0;
 }
 
@@ -589,7 +578,7 @@ extern "C" int bjx_chees_update(bjx_handle_t h, void* nccl_comm, int32_t n_ranks
       !step_size_chain || !steps_chain)
     return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   const int nb = n_stat_blocks(C);
   const size_t S1 = 3 + 3 * (size_t)D;
@@ -604,7 +593,7 @@ extern "C" int bjx_chees_update(bjx_handle_t h, void* nccl_comm, int32_t n_ranks
   k_chees_w<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, acceptance_rate, is_divergent, w);
   k_chees_pass1<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, proposal_position, initial_position, acceptance_rate,
                                                               is_divergent, w, loc1);
-  AD_LAUNCH("k_chees_pass1");
+  BJX_CHECK_LAUNCH("k_chees_pass1");
   const float* m1 = loc1;
   if (n_ranks > 1) {
     int rc = bjx_allgather_stats(h, nccl_comm, loc1, (int64_t)(nb * S1), gat1);
@@ -615,7 +604,7 @@ extern "C" int bjx_chees_update(bjx_handle_t h, void* nccl_comm, int32_t n_ranks
   k_chees_dots<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, proposal_momentum, initial_position, acceptance_rate,
                                           is_divergent, state, num, den);
   k_chees_pass2<<<nb, 256, 0, s>>>(C, num, den, loc2);
-  AD_LAUNCH("k_chees_pass2");
+  BJX_CHECK_LAUNCH("k_chees_pass2");
   const float* m2 = loc2;
   if (n_ranks > 1) {
     int rc = bjx_allgather_stats(h, nccl_comm, loc2, (int64_t)(nb * 2), gat2);
@@ -626,16 +615,16 @@ extern "C" int bjx_chees_update(bjx_handle_t h, void* nccl_comm, int32_t n_ranks
                                   (float)max_leapfrog_steps, history);
   k_fill_from<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_EPS, step_size_chain);
   k_fill_steps<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_L, steps_chain);
-  AD_LAUNCH("k_chees_finish");
+  BJX_CHECK_LAUNCH("k_chees_finish");
   return 0;
 }
 
 extern "C" int bjx_chees_final(bjx_handle_t h, const float* state, float* out2) {
   if (!h || !state || !out2) return bjx_fail(h, BJX_E_INVALID, "null argument");
-  AD_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   float hst[kChHdr];
-  AD_CUDA(cudaMemcpyAsync(hst, state, sizeof(hst), cudaMemcpyDeviceToHost, h->stream));
-  AD_CUDA(cudaStreamSynchronize(h->stream));
+  BJX_CUDA(cudaMemcpyAsync(hst, state, sizeof(hst), cudaMemcpyDeviceToHost, h->stream));
+  BJX_CUDA(cudaStreamSynchronize(h->stream));
   out2[0] = expf(hst[CH_LOG_EPS_MA]);                       // step_size
   out2[1] = expf(hst[CH_LOG_T_MA] - hst[CH_LOG_EPS_MA]);    // num_leapfrog_steps (integration_steps_params)
   return 0;

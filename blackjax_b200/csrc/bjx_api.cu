@@ -27,8 +27,6 @@ int bjx_fail(bjx_handle_t h, int code, const std::string& msg) {
 int bjx_cuda_fail(bjx_handle_t h, cudaError_t e, const char* where) {
   return bjx_fail(h, (int)e, std::string(where) + ": " + cudaGetErrorString(e));
 }
-static int fail(bjx_handle_t h, int code, const std::string& msg) { return bjx_fail(h, code, msg); }
-static int cuda_fail(bjx_handle_t h, cudaError_t e, const char* where) { return bjx_cuda_fail(h, e, where); }
 
 // large-D dense path (bjx_dense.cu)
 int bjx_dense_init_state(bjx_handle_t h, const float* q, float* logp_out, float* grad_out);
@@ -43,11 +41,6 @@ int bjx_dense_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* q_in,
                         float* q_out, float* logp_out, float* g_out, float step_size, const float* step_size_dev,
                         int max_num_doublings, bjx::InfoPtrs info, const float* momentum_override,
                         const uint32_t* key_integrator_override);
-static inline bool target_large_dense(bjx_handle_t h) {
-  return h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN && h->cfg.dim > 128;
-}
-static inline bool metric_large_dense(bjx_handle_t h) { return h->metric_kind == BJX_METRIC_DENSE && h->cfg.dim > 128; }
-static inline bool use_dense_path(bjx_handle_t h) { return target_large_dense(h) || metric_large_dense(h); }
 
 // CTA-per-chain path for 1024 < dim <= 18432 (bjx_big.cu)
 int bjx_big_init_state(bjx_handle_t h, const float* q, float* logp_out, float* grad_out);
@@ -57,80 +50,87 @@ int bjx_big_leapfrog(bjx_handle_t h, float* q, float* p, float* logp, float* g, 
 int bjx_big_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, const float* g_in,
                      float* q_out, float* logp_out, float* g_out, float eps, const float* eps_dev, int L,
                      const bjx::InfoPtrs& info);
-static inline bool use_big_path(bjx_handle_t h) { return h->sc == SC_BIG && !use_dense_path(h); }
-#define BJX_CUDA(call)                                            \
-  do {                                                            \
-    cudaError_t e_ = (call);                                      \
-    if (e_ != cudaSuccess) return cuda_fail(h, e_, #call);        \
-  } while (0)
-#define BJX_CHECK_LAUNCH(where)                                   \
-  do {                                                            \
-    cudaError_t e_ = cudaGetLastError();                          \
-    if (e_ != cudaSuccess) return cuda_fail(h, e_, where);        \
-  } while (0)
+
+// Execution path of a call.  ROUTE_ROWS: the warp-per-chain row kernels (dim <= 1024, bjx_launch.cuh); ROUTE_BIG: the
+// CTA-per-chain kernels (1024 < dim, bjx_big.cu); ROUTE_DENSE: the tensor-core dense path (bjx_dense.cu), taken by a dense
+// Gaussian target or a dense metric beyond 128 dims.
+enum Route { ROUTE_ROWS, ROUTE_BIG, ROUTE_DENSE };
+static Route rows_or_big(bjx_handle_t h) { return h->sc == SC_BIG ? ROUTE_BIG : ROUTE_ROWS; }
+// where the target alone is evaluated (bjx_init_state)
+static Route target_route(bjx_handle_t h) {
+  if (h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN && h->cfg.dim > 128) return ROUTE_DENSE;
+  return rows_or_big(h);
+}
+// where the metric alone is applied (momentum draw, kinetic energy, U-turn test)
+static Route metric_route(bjx_handle_t h) {
+  if (h->metric_kind == BJX_METRIC_DENSE && h->cfg.dim > 128) return ROUTE_DENSE;
+  return rows_or_big(h);
+}
+// where a transition, which needs both, runs
+static Route transition_route(bjx_handle_t h) {
+  if (target_route(h) == ROUTE_DENSE || metric_route(h) == ROUTE_DENSE) return ROUTE_DENSE;
+  return rows_or_big(h);
+}
 
 static int validate_target(bjx_handle_t h, const bjx_target_desc& t, int dim) {
-  if (t.dim != dim) return fail(h, BJX_E_INVALID, "target.dim != config.dim");
+  if (t.dim != dim) return bjx_fail(h, BJX_E_INVALID, "target.dim != config.dim");
   switch (t.kind) {
     case BJX_TARGET_DIAG_GAUSSIAN:
-      if (!t.inv_var) return fail(h, BJX_E_INVALID, "DIAG_GAUSSIAN target needs inv_var");
+      if (!t.inv_var) return bjx_fail(h, BJX_E_INVALID, "DIAG_GAUSSIAN target needs inv_var");
       break;
     case BJX_TARGET_FUNNEL:
-      if (dim < 2) return fail(h, BJX_E_INVALID, "FUNNEL target needs dim >= 2");
+      if (dim < 2) return bjx_fail(h, BJX_E_INVALID, "FUNNEL target needs dim >= 2");
       break;
     case BJX_TARGET_DENSE_GAUSSIAN:
-      if (!t.precision) return fail(h, BJX_E_INVALID, "DENSE_GAUSSIAN target needs precision");
-      if (dim > 128 && dim % 4 != 0) return fail(h, BJX_E_UNSUPPORTED, "DENSE_GAUSSIAN target with dim > 128 needs dim % 4 == 0 (tensor-core GEMM path)");
+      if (!t.precision) return bjx_fail(h, BJX_E_INVALID, "DENSE_GAUSSIAN target needs precision");
+      if (dim > 128 && dim % 4 != 0) return bjx_fail(h, BJX_E_UNSUPPORTED, "DENSE_GAUSSIAN target with dim > 128 needs dim % 4 == 0 (tensor-core GEMM path)");
       break;
     case BJX_TARGET_BANANA:
-      if (dim != 2) return fail(h, BJX_E_INVALID, "BANANA target needs dim == 2");
+      if (dim != 2) return bjx_fail(h, BJX_E_INVALID, "BANANA target needs dim == 2");
       break;
     case BJX_TARGET_HIER_LOGIT:
       if (!t.data_x || !t.data_y || t.n_groups < 1 || dim != 4 + t.n_groups)
-        return fail(h, BJX_E_INVALID, "HIER_LOGIT target needs data_x, data_y and dim == 4 + n_groups");
+        return bjx_fail(h, BJX_E_INVALID, "HIER_LOGIT target needs data_x, data_y and dim == 4 + n_groups");
       if (dim <= 1024 || dim % 4 != 0)
-        return fail(h, BJX_E_UNSUPPORTED, "HIER_LOGIT target is built for 1024 < dim <= 18432, dim % 4 == 0 (CTA-per-chain kernels)");
+        return bjx_fail(h, BJX_E_UNSUPPORTED, "HIER_LOGIT target is built for 1024 < dim <= 18432, dim % 4 == 0 (CTA-per-chain kernels)");
       break;
     case BJX_TARGET_USER:
-      if (!t.user_plugin) return fail(h, BJX_E_INVALID, "USER target needs user_plugin (bjx_plugin_load)");
+      if (!t.user_plugin) return bjx_fail(h, BJX_E_INVALID, "USER target needs user_plugin (bjx_plugin_load)");
       if (t.n_user_params < 0 || (t.n_user_params > 0 && !t.user_params))
-        return fail(h, BJX_E_INVALID, "USER target: user_params is NULL but n_user_params > 0");
+        return bjx_fail(h, BJX_E_INVALID, "USER target: user_params is NULL but n_user_params > 0");
       {
         auto* pl = static_cast<bjx_plugin_s*>(t.user_plugin);
         if (dim > 1024 && !pl->launch_big)
-          return fail(h, BJX_E_UNSUPPORTED, "this USER target's plug-in holds the warp kernels only (dim <= 1024): build it with "
-                                            "bjx_user::BigModel for rows beyond");
+          return bjx_fail(h, BJX_E_UNSUPPORTED, "this USER target's plug-in holds the warp kernels only (dim <= 1024): build it with "
+                                                "bjx_user::BigModel for rows beyond");
         if (dim <= 1024 && !pl->launch)
-          return fail(h, BJX_E_UNSUPPORTED, "this USER target's plug-in holds the big-row kernels only (dim > 1024)");
+          return bjx_fail(h, BJX_E_UNSUPPORTED, "this USER target's plug-in holds the big-row kernels only (dim > 1024)");
       }
       break;
     default:
-      return fail(h, BJX_E_INVALID, "unknown target kind");
+      return bjx_fail(h, BJX_E_INVALID, "unknown target kind");
   }
   return 0;
 }
 
 // ---- plug-ins of user-defined targets (include/bjx_user_target.h) ---------------------------------------------------
-// what a plug-in must have been built against: the C ABI version and the layout of the launch arguments
-extern "C" int bjx_plugin_abi(void) {
-  return BJX_VERSION * 100000 + (int)sizeof(bjx::LaunchArgs) + 7 * (int)sizeof(bjx::BigLaunchArgs);
-}
+extern "C" int bjx_plugin_abi(void) { return plugin_abi(); }
 
 extern "C" int bjx_plugin_load(const char* path, void** plugin_out) {
-  if (!path || !plugin_out) return fail(nullptr, BJX_E_INVALID, "null argument");
+  if (!path || !plugin_out) return bjx_fail(nullptr, BJX_E_INVALID, "null argument");
   void* dl = dlopen(path, RTLD_NOW | RTLD_LOCAL);
-  if (!dl) return fail(nullptr, BJX_E_INVALID, std::string("bjx_plugin_load: ") + dlerror());
+  if (!dl) return bjx_fail(nullptr, BJX_E_INVALID, std::string("bjx_plugin_load: ") + dlerror());
   auto abi = (int (*)(void))dlsym(dl, "bjx_plugin_built_for_abi");
   auto launch = (int (*)(int, int, int, const bjx::LaunchArgs*))dlsym(dl, "bjx_plugin_launch");
   auto launch_big = (int (*)(int, const bjx::BigLaunchArgs*))dlsym(dl, "bjx_plugin_launch_big");
   if (!abi || (!launch && !launch_big)) {
     dlclose(dl);
-    return fail(nullptr, BJX_E_INVALID, std::string("bjx_plugin_load: ") + path + " is not a bjx target plug-in");
+    return bjx_fail(nullptr, BJX_E_INVALID, std::string("bjx_plugin_load: ") + path + " is not a bjx target plug-in");
   }
   if (abi() != bjx_plugin_abi()) {
     dlclose(dl);
-    return fail(nullptr, BJX_E_STATE, std::string("bjx_plugin_load: ") + path +
-                                          " was built against another version of libbjx's kernels: rebuild it");
+    return bjx_fail(nullptr, BJX_E_STATE, std::string("bjx_plugin_load: ") + path +
+                                              " was built against another version of libbjx's kernels: rebuild it");
   }
   *plugin_out = new bjx_plugin_s{dl, launch, launch_big};  // never unloaded: handles may refer to it until the process ends
   return 0;
@@ -141,70 +141,29 @@ extern "C" int bjx_version(void) { return BJX_VERSION; }
 extern "C" const char* bjx_last_error(bjx_handle_t h) { return h ? h->err.c_str() : g_err.c_str(); }
 
 extern "C" int bjx_create(const bjx_config* cfg, bjx_handle_t* out) {
-  bjx_handle_t h = nullptr;
-  if (!cfg || !out) return fail(nullptr, BJX_E_INVALID, "null argument");
-  if (cfg->n_chains <= 0 || cfg->dim <= 0) return fail(nullptr, BJX_E_INVALID, "n_chains and dim must be positive");
-  if (cfg->max_tree_depth < 1 || cfg->max_tree_depth > 30) return fail(nullptr, BJX_E_INVALID, "max_tree_depth must be in [1, 30]");
+  if (!cfg || !out) return bjx_fail(nullptr, BJX_E_INVALID, "null argument");
+  if (cfg->n_chains <= 0 || cfg->dim <= 0) return bjx_fail(nullptr, BJX_E_INVALID, "n_chains and dim must be positive");
+  if (cfg->max_tree_depth < 1 || cfg->max_tree_depth > 30) return bjx_fail(nullptr, BJX_E_INVALID, "max_tree_depth must be in [1, 30]");
   const int sc = size_class_for(cfg->dim);
   if (sc == SC_NONE)
-    return fail(nullptr, BJX_E_UNSUPPORTED, "dim must be <= 18432 with dim % 4 == 0, or <= 128 otherwise");
+    return bjx_fail(nullptr, BJX_E_UNSUPPORTED, "dim must be <= 18432 with dim % 4 == 0, or <= 128 otherwise");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaGetDeviceCount (no CUDA device: there is no CPU fallback)");
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(nullptr, BJX_E_INVALID, "bad device ordinal");
+  if (e != cudaSuccess) return bjx_cuda_fail(nullptr, e, "cudaGetDeviceCount (no CUDA device: there is no CPU fallback)");
+  if (cfg->device < 0 || cfg->device >= ndev) return bjx_fail(nullptr, BJX_E_INVALID, "bad device ordinal");
   e = cudaSetDevice(cfg->device);
-  if (e != cudaSuccess) return cuda_fail(nullptr, e, "cudaSetDevice");
-  h = new bjx_handle_s();
+  if (e != cudaSuccess) return bjx_cuda_fail(nullptr, e, "cudaSetDevice");
+  int rc = validate_target(nullptr, cfg->target, cfg->dim);
+  if (rc) return rc;
+  int* h_flag = nullptr;
+  e = cudaMallocHost((void**)&h_flag, 64 * sizeof(int));
+  if (e != cudaSuccess) return bjx_cuda_fail(nullptr, e, "cudaMallocHost");
+  bjx_handle_t h = new bjx_handle_s();  // (defaults: bjx_handle.h)
   h->cfg = *cfg;
   if (!(h->cfg.divergence_threshold > 0.f)) h->cfg.divergence_threshold = 1000.f;
   h->stream = (cudaStream_t)cfg->stream;
   h->sc = sc;
-  h->metric_kind = -1;
-  h->metric_small_dense = false;
-  h->imm = nullptr;
-  h->msqrt = nullptr;
-  h->msqrt_elems = 0;
-  memset(&h->ws, 0, sizeof(h->ws));
-  h->ws_block = nullptr;
-  h->ws_depth = 0;
-  h->h_flag = nullptr;
-  h->last_leaf_launches = 0;
-  h->last_depth = 0;
-  h->dense_block = nullptr;
-  h->dense_bytes = 0;
-  h->gemm_ws = nullptr;
-  h->gemm_ws_bytes = 0;
-  for (int m = 0; m < 3; ++m) { h->dense_mat_s[m] = nullptr; h->dense_mat_src[m] = nullptr; h->dense_mat_ver[m] = 0; }
-  h->dense_version = 1;
-  h->dense_bytes_built = 0;
-  h->pool_scratch = nullptr;
-  h->dn_block = nullptr;
-  h->dn_bytes = 0;
-  h->pool_scratch_bytes = 0;
-  h->lr_block = nullptr;
-  h->lr_k = 0;
-  h->dense_streams_ready = false;
-  h->dense_stagger_armed = false;
-  h->ncoef = 3;
-  h->coef[0] = 0.5f; h->coef[1] = 1.0f; h->coef[2] = 0.5f;
-  h->general_integrator = false;
-  h->key_shared = 0;
-  h->steps_dev = nullptr;
-  h->ghmc_noise = nullptr;
-  h->chain_offset = 0;
-  h->sample_keys = nullptr;
-  h->sample_keys_cap = 0;
-  int rc = validate_target(h, cfg->target, cfg->dim);
-  if (rc) {
-    g_err = h->err;
-    delete h;
-    return rc;
-  }
-  e = cudaMallocHost((void**)&h->h_flag, 64 * sizeof(int));
-  if (e != cudaSuccess) {
-    delete h;
-    return cuda_fail(nullptr, e, "cudaMallocHost");
-  }
+  h->h_flag = h_flag;
   *out = h;
   return 0;
 }
@@ -221,18 +180,13 @@ extern "C" int bjx_destroy(bjx_handle_t h) {
   if (h->lr_block) cudaFree(h->lr_block);
   if (h->gemm_ws) cudaFree(h->gemm_ws);
   if (h->sample_keys) cudaFree(h->sample_keys);
-  if (h->dense_streams_ready) {
-    for (int k = 0; k < 2; ++k) { cudaStreamDestroy(h->dense_stream[k]); cudaEventDestroy(h->dense_join[k]); }
-    cudaEventDestroy(h->dense_fork);
-    cudaEventDestroy(h->dense_stagger);
-  }
   if (h->h_flag) cudaFreeHost(h->h_flag);
   delete h;
   return 0;
 }
 
 extern "C" int bjx_set_target(bjx_handle_t h, const bjx_target_desc* t) {
-  if (!h || !t) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !t) return bjx_fail(h, BJX_E_INVALID, "null argument");
   int rc = validate_target(h, *t, h->cfg.dim);
   if (rc) return rc;
   h->cfg.target = *t;
@@ -242,10 +196,10 @@ extern "C" int bjx_set_target(bjx_handle_t h, const bjx_target_desc* t) {
 
 // integrators.py:62-152,321-369: palindromic coefficient table (host array, odd length 3..11)
 extern "C" int bjx_set_integrator(bjx_handle_t h, const float* coefficients, int32_t n) {
-  if (!h || !coefficients) return fail(h, BJX_E_INVALID, "null argument");
-  if (n < 3 || n > 11 || (n % 2) == 0) return fail(h, BJX_E_INVALID, "integrator needs an odd number (3..11) of coefficients");
+  if (!h || !coefficients) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (n < 3 || n > 11 || (n % 2) == 0) return bjx_fail(h, BJX_E_INVALID, "integrator needs an odd number (3..11) of coefficients");
   for (int i = 0; i < n; ++i)
-    if (coefficients[i] != coefficients[n - 1 - i]) return fail(h, BJX_E_INVALID, "integrator coefficients must be palindromic");
+    if (coefficients[i] != coefficients[n - 1 - i]) return bjx_fail(h, BJX_E_INVALID, "integrator coefficients must be palindromic");
   h->ncoef = n;
   for (int i = 0; i < n; ++i) h->coef[i] = coefficients[i];
   h->general_integrator = !(n == 3 && coefficients[0] == 0.5f && coefficients[1] == 1.0f);
@@ -255,7 +209,7 @@ extern "C" int bjx_set_integrator(bjx_handle_t h, const float* coefficients, int
 // Key source of the transition kernels: 0 = `keys` holds one key per chain [C,2]; 1 = `keys` holds ONE step key [2] and
 // chain c uses split(step_key, n_global)[chain_offset + c] (util.py:203 / staged_adaptation.py:920 step-major schedule).
 extern "C" int bjx_set_key_mode(bjx_handle_t h, int32_t shared_step_key, uint32_t chain_offset) {
-  if (!h) return fail(h, BJX_E_INVALID, "null handle");
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
   h->key_shared = shared_step_key ? 1 : 0;
   h->chain_offset = chain_offset;
   return 0;
@@ -264,7 +218,7 @@ extern "C" int bjx_set_key_mode(bjx_handle_t h, int32_t shared_step_key, uint32_
 // Dynamic HMC (blackjax/mcmc/dynamic_hmc.py:109-120): per-chain numbers of integration steps int32 [C] (device) for the
 // following bjx_hmc_step / bjx_mhmc_step calls, whose scalar L is then ignored; NULL restores the scalar.
 extern "C" int bjx_set_integration_steps(bjx_handle_t h, const int32_t* steps_dev) {
-  if (!h) return fail(h, BJX_E_INVALID, "null handle");
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
   h->steps_dev = steps_dev;
   return 0;
 }
@@ -272,40 +226,36 @@ extern "C" int bjx_set_integration_steps(bjx_handle_t h, const int32_t* steps_de
 // Generalized HMC's slice noise (blackjax/mcmc/ghmc.py:90,172 `noise_fn(key_noise)`): per-chain values float32 [C]
 // (device) added to the slice translation of the following bjx_ghmc_step calls; NULL restores the default (0).
 extern "C" int bjx_set_ghmc_noise(bjx_handle_t h, const float* noise_dev) {
-  if (!h) return fail(h, BJX_E_INVALID, "null handle");
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
   h->ghmc_noise = noise_dev;
   return 0;
 }
 
 extern "C" int bjx_synchronize(bjx_handle_t h) {
-  if (!h) return fail(h, BJX_E_INVALID, "null handle");
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   BJX_CUDA(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
 extern "C" int bjx_set_metric(bjx_handle_t h, int32_t kind, const float* imm) {
-  if (!h || !imm) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !imm) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int D = h->cfg.dim, C = h->cfg.n_chains;
   size_t elems;
   if (kind == BJX_METRIC_DIAG) elems = D;
   else if (kind == BJX_METRIC_DIAG_PER_CHAIN) elems = (size_t)C * D;
   else if (kind == BJX_METRIC_DENSE_PER_CHAIN) {
-    if (D > 64) return fail(h, BJX_E_UNSUPPORTED, "per-chain dense metrics are built for dim <= 64");
+    if (D > 64) return bjx_fail(h, BJX_E_UNSUPPORTED, "per-chain dense metrics are built for dim <= 64");
     elems = (size_t)C * D * D;
   } else if (kind == BJX_METRIC_DENSE) {
     if (D > 128 && D % 4 != 0)
-      return fail(h, BJX_E_UNSUPPORTED, "dense metric with dim > 128 needs dim % 4 == 0 (tensor-core GEMM path)");
+      return bjx_fail(h, BJX_E_UNSUPPORTED, "dense metric with dim > 128 needs dim % 4 == 0 (tensor-core GEMM path)");
     elems = (size_t)D * D;
   } else
-    return fail(h, BJX_E_INVALID, "The mass matrix has the wrong number of dimensions: expected 1 or 2");  // metrics.py:724-728
-  if (elems > h->msqrt_elems) {
-    if (h->msqrt) BJX_CUDA(cudaFree(h->msqrt));
-    h->msqrt = nullptr;
-    BJX_CUDA(cudaMalloc((void**)&h->msqrt, elems * sizeof(float)));
-    h->msqrt_elems = elems;
-  }
+    return bjx_fail(h, BJX_E_INVALID, "The mass matrix has the wrong number of dimensions: expected 1 or 2");  // metrics.py:724-728
+  int rc = bjx_grow(h, h->msqrt, h->msqrt_elems, elems, sizeof(float));
+  if (rc) return rc;
   if (kind == BJX_METRIC_DENSE) {
     // metrics.py:712-715: L = chol(M^-1) (lower); mass_matrix_sqrt = solve_triangular(L, I, lower, trans) = L^-T
     std::vector<float> a((size_t)D * D);
@@ -317,7 +267,7 @@ extern "C" int bjx_set_metric(bjx_handle_t h, int32_t kind, const float* imm) {
         double s = a[(size_t)i * D + j];
         for (int k = 0; k < j; ++k) s -= L[(size_t)i * D + k] * L[(size_t)j * D + k];
         if (i == j) {
-          if (!(s > 0.0)) return fail(h, BJX_E_INVALID, "inverse mass matrix is not positive definite");
+          if (!(s > 0.0)) return bjx_fail(h, BJX_E_INVALID, "inverse mass matrix is not positive definite");
           L[(size_t)i * D + i] = sqrt(s);
         } else
           L[(size_t)i * D + j] = s / L[(size_t)j * D + j];
@@ -363,11 +313,11 @@ static __global__ void k_low_rank_prepare(int D, int k, const float* __restrict_
 }
 
 extern "C" int bjx_set_metric_low_rank(bjx_handle_t h, const float* sigma, const float* U, const float* lam, int32_t rank) {
-  if (!h || !sigma || !U || !lam) return fail(h, BJX_E_INVALID, "null argument");
-  if (rank < 1 || rank > kMaxLowRank) return fail(h, BJX_E_UNSUPPORTED, "low-rank metric: 1 <= rank <= 16");
+  if (!h || !sigma || !U || !lam) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (rank < 1 || rank > kMaxLowRank) return bjx_fail(h, BJX_E_UNSUPPORTED, "low-rank metric: 1 <= rank <= 16");
   const int D = h->cfg.dim;
-  if (h->sc == SC_BIG || h->sc == SC_V8 || h->sc == SC_NONE || use_dense_path(h))
-    return fail(h, BJX_E_UNSUPPORTED, "low-rank metric is built for the warp kernels with dim <= 512 (dim % 4 == 0 above 128)");
+  if (transition_route(h) != ROUTE_ROWS || h->sc == SC_V8)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "low-rank metric is built for the warp kernels with dim <= 512 (dim % 4 == 0 above 128)");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   const size_t need = ((size_t)D * rank + 2 * (size_t)D + 2 * (size_t)rank) * sizeof(float);
   if (h->lr_block) BJX_CUDA(cudaFree(h->lr_block));
@@ -387,8 +337,8 @@ extern "C" int bjx_set_metric_low_rank(bjx_handle_t h, const float* sigma, const
 }
 
 extern "C" int bjx_get_mass_matrix_sqrt(bjx_handle_t h, const float** out) {
-  if (!h || !out) return fail(h, BJX_E_INVALID, "null argument");
-  if (h->metric_kind < 0) return fail(h, BJX_E_STATE, "metric not set");
+  if (!h || !out) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (h->metric_kind < 0) return bjx_fail(h, BJX_E_STATE, "metric not set");
   *out = h->msqrt;
   return 0;
 }
@@ -444,24 +394,32 @@ static int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, Launch
     case BJX_TARGET_USER:
       if (!static_cast<bjx_plugin_s*>(h->cfg.target.user_plugin)->launch) { rc = -2; break; }
       rc = static_cast<bjx_plugin_s*>(h->cfg.target.user_plugin)->launch(kernel_id, h->sc, dm ? 1 : 0, &a);
-      if (rc > 0) return cuda_fail(h, (cudaError_t)rc, "plug-in kernel launch");
+      if (rc > 0) return bjx_cuda_fail(h, (cudaError_t)rc, "plug-in kernel launch");
       break;
     default: rc = -2;
   }
-  if (rc) return fail(h, BJX_E_UNSUPPORTED, "kernel variant not built for this (target, dim, metric, integrator) combination");
+  if (rc) return bjx_fail(h, BJX_E_UNSUPPORTED, "kernel variant not built for this (target, dim, metric, integrator) combination");
   BJX_CHECK_LAUNCH("kernel launch");
   return 0;
 }
 
 static int check_ready(bjx_handle_t h, bool need_metric, const void* const* ptrs, int n) {
-  if (!h) return fail(h, BJX_E_INVALID, "null handle");
-  if (need_metric && h->metric_kind < 0) return fail(h, BJX_E_STATE, "metric not set: call bjx_set_metric first");
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
+  if (need_metric && h->metric_kind < 0) return bjx_fail(h, BJX_E_STATE, "metric not set: call bjx_set_metric first");
   for (int i = 0; i < n; ++i) {
-    if (!ptrs[i]) return fail(h, BJX_E_INVALID, "null array argument");
-    if (size_class_is_vec(h->sc) && ((uintptr_t)ptrs[i] & 15u)) return fail(h, BJX_E_INVALID, "state arrays must be 16-byte aligned");
+    if (!ptrs[i]) return bjx_fail(h, BJX_E_INVALID, "null array argument");
+    if (size_class_is_vec(h->sc) && ((uintptr_t)ptrs[i] & 15u)) return bjx_fail(h, BJX_E_INVALID, "state arrays must be 16-byte aligned");
   }
   cudaError_t e = cudaSetDevice(h->cfg.device);
-  if (e != cudaSuccess) return cuda_fail(h, e, "cudaSetDevice");
+  if (e != cudaSuccess) return bjx_cuda_fail(h, e, "cudaSetDevice");
+  return 0;
+}
+
+// In-place transitions alias all of (q, logp, grad) or none of them.
+static int check_in_place(bjx_handle_t h, const float* q_in, const float* logp_in, const float* g_in, const float* q_out,
+                          const float* logp_out, const float* g_out) {
+  if ((q_in == q_out) != (g_in == g_out) || (q_in == q_out) != (logp_in == logp_out))
+    return bjx_fail(h, BJX_E_INVALID, "in-place call must alias all of (q, logp, grad)");
   return 0;
 }
 
@@ -469,9 +427,12 @@ extern "C" int bjx_init_state(bjx_handle_t h, const float* q, float* logp_out, f
   const void* ptrs[] = {q, grad_out};
   int rc = check_ready(h, false, ptrs, 2);
   if (rc) return rc;
-  if (!logp_out) return fail(h, BJX_E_INVALID, "null array argument");
-  if (target_large_dense(h)) return bjx_dense_init_state(h, q, logp_out, grad_out);
-  if (h->sc == SC_BIG) return bjx_big_init_state(h, q, logp_out, grad_out);
+  if (!logp_out) return bjx_fail(h, BJX_E_INVALID, "null array argument");
+  switch (target_route(h)) {
+    case ROUTE_DENSE: return bjx_dense_init_state(h, q, logp_out, grad_out);
+    case ROUTE_BIG: return bjx_big_init_state(h, q, logp_out, grad_out);
+    case ROUTE_ROWS: break;
+  }
   LaunchArgs a{};
   a.P = make_params(h, 0.f, nullptr);
   a.q_in = q;
@@ -485,9 +446,12 @@ extern "C" int bjx_sample_momentum(bjx_handle_t h, const uint32_t* keys, float* 
   const void* ptrs[] = {p_out};
   int rc = check_ready(h, true, ptrs, 1);
   if (rc) return rc;
-  if (!keys) return fail(h, BJX_E_INVALID, "null keys");
-  if (metric_large_dense(h)) return bjx_dense_sample_momentum(h, keys, p_out, false);
-  if (h->sc == SC_BIG) return bjx_big_sample_momentum(h, keys, p_out);
+  if (!keys) return bjx_fail(h, BJX_E_INVALID, "null keys");
+  switch (metric_route(h)) {
+    case ROUTE_DENSE: return bjx_dense_sample_momentum(h, keys, p_out, false);
+    case ROUTE_BIG: return bjx_big_sample_momentum(h, keys, p_out);
+    case ROUTE_ROWS: break;
+  }
   LaunchArgs a{};
   a.P = make_params(h, 0.f, nullptr);
   a.keys = keys;
@@ -500,11 +464,15 @@ extern "C" int bjx_leapfrog(bjx_handle_t h, float* q, float* p, float* logp, flo
   const void* ptrs[] = {q, p, grad};
   int rc = check_ready(h, true, ptrs, 3);
   if (rc) return rc;
-  if (!logp || n_steps < 0) return fail(h, BJX_E_INVALID, "bad argument");
-  if ((use_dense_path(h) || use_big_path(h)) && h->general_integrator)
-    return fail(h, BJX_E_UNSUPPORTED, "only velocity Verlet is built for dim > 1024 / the tensor-core dense path");
-  if (use_dense_path(h)) return bjx_dense_leapfrog(h, q, p, logp, grad, step_size, step_size_dev, n_steps);
-  if (use_big_path(h)) return bjx_big_leapfrog(h, q, p, logp, grad, step_size, step_size_dev, n_steps);
+  if (!logp || n_steps < 0) return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  const Route route = transition_route(h);
+  if (route != ROUTE_ROWS && h->general_integrator)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "only velocity Verlet is built for dim > 1024 / the tensor-core dense path");
+  switch (route) {
+    case ROUTE_DENSE: return bjx_dense_leapfrog(h, q, p, logp, grad, step_size, step_size_dev, n_steps);
+    case ROUTE_BIG: return bjx_big_leapfrog(h, q, p, logp, grad, step_size, step_size_dev, n_steps);
+    case ROUTE_ROWS: break;
+  }
   LaunchArgs a{};
   a.P = make_params(h, step_size, step_size_dev);
   a.q_out = q;
@@ -520,19 +488,22 @@ extern "C" int bjx_metric_velocity(bjx_handle_t h, const float* p, float* v_out)
   int rc = check_ready(h, true, ptrs, 2);
   if (rc) return rc;
   if (h->cfg.dim > 128) {
-    if (h->cfg.dim % 4) return fail(h, BJX_E_UNSUPPORTED, "bjx_metric_velocity needs dim % 4 == 0 for dim > 128");
+    if (h->cfg.dim % 4) return bjx_fail(h, BJX_E_UNSUPPORTED, "bjx_metric_velocity needs dim % 4 == 0 for dim > 128");
     return bjx_dense_velocity(h, p, v_out);
   }
-  return fail(h, BJX_E_UNSUPPORTED, "bjx_metric_velocity is built for dim > 128 (use bjx_energy / bjx_leapfrog below)");
+  return bjx_fail(h, BJX_E_UNSUPPORTED, "bjx_metric_velocity is built for dim > 128 (use bjx_energy / bjx_leapfrog below)");
 }
 
 extern "C" int bjx_energy(bjx_handle_t h, const float* p, const float* logp, float* energy_out) {
   const void* ptrs[] = {p};
   int rc = check_ready(h, true, ptrs, 1);
   if (rc) return rc;
-  if (!logp || !energy_out) return fail(h, BJX_E_INVALID, "null array argument");
-  if (metric_large_dense(h)) return bjx_dense_energy(h, p, logp, energy_out);
-  if (h->sc == SC_BIG) return bjx_big_energy(h, p, logp, energy_out);
+  if (!logp || !energy_out) return bjx_fail(h, BJX_E_INVALID, "null array argument");
+  switch (metric_route(h)) {
+    case ROUTE_DENSE: return bjx_dense_energy(h, p, logp, energy_out);
+    case ROUTE_BIG: return bjx_big_energy(h, p, logp, energy_out);
+    case ROUTE_ROWS: break;
+  }
   LaunchArgs a{};
   a.P = make_params(h, 0.f, nullptr);
   a.p_io = const_cast<float*>(p);
@@ -545,9 +516,12 @@ extern "C" int bjx_is_turning(bjx_handle_t h, const float* pl, const float* pr, 
   const void* ptrs[] = {pl, pr, ps};
   int rc = check_ready(h, true, ptrs, 3);
   if (rc) return rc;
-  if (!out) return fail(h, BJX_E_INVALID, "null array argument");
-  if (metric_large_dense(h)) return fail(h, BJX_E_UNSUPPORTED, "U-turn test with a dense metric needs dim <= 128");
-  if (h->sc == SC_BIG) return fail(h, BJX_E_UNSUPPORTED, "U-turn test / NUTS are built for dim <= 1024");
+  if (!out) return bjx_fail(h, BJX_E_INVALID, "null array argument");
+  switch (metric_route(h)) {
+    case ROUTE_DENSE: return bjx_fail(h, BJX_E_UNSUPPORTED, "U-turn test with a dense metric needs dim <= 128");
+    case ROUTE_BIG: return bjx_fail(h, BJX_E_UNSUPPORTED, "U-turn test / NUTS are built for dim <= 1024");
+    case ROUTE_ROWS: break;
+  }
   LaunchArgs a{};
   a.P = make_params(h, 0.f, nullptr);
   a.pl = pl;
@@ -580,19 +554,23 @@ extern "C" int bjx_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q
   const void* ptrs[] = {q_in, grad_in, q_out, grad_out};
   int rc = check_ready(h, true, ptrs, 4);
   if (rc) return rc;
-  if (!keys || !logp_in || !logp_out || L < 0) return fail(h, BJX_E_INVALID, "bad argument");
-  if ((q_in == q_out) != (grad_in == grad_out) || (q_in == q_out) != (logp_in == logp_out))
-    return fail(h, BJX_E_INVALID, "in-place call must alias all of (q, logp, grad)");
-  if ((use_dense_path(h) || use_big_path(h)) && h->general_integrator)
-    return fail(h, BJX_E_UNSUPPORTED, "only velocity Verlet is built for dim > 1024 / the tensor-core dense path");
-  if ((use_dense_path(h) || use_big_path(h)) && h->steps_dev)
-    return fail(h, BJX_E_UNSUPPORTED, "per-chain integration steps need dim <= 1024 and the row-resident kernels");
-  if (use_dense_path(h))
-    return bjx_dense_hmc_step(h, keys, q_in, logp_in, grad_in, q_out, logp_out, grad_out, step_size, step_size_dev, L,
+  if (!keys || !logp_in || !logp_out || L < 0) return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  rc = check_in_place(h, q_in, logp_in, grad_in, q_out, logp_out, grad_out);
+  if (rc) return rc;
+  const Route route = transition_route(h);
+  if (route != ROUTE_ROWS && h->general_integrator)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "only velocity Verlet is built for dim > 1024 / the tensor-core dense path");
+  if (route != ROUTE_ROWS && h->steps_dev)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "per-chain integration steps need dim <= 1024 and the row-resident kernels");
+  switch (route) {
+    case ROUTE_DENSE:
+      return bjx_dense_hmc_step(h, keys, q_in, logp_in, grad_in, q_out, logp_out, grad_out, step_size, step_size_dev, L,
+                                make_info(info));
+    case ROUTE_BIG:
+      return bjx_big_hmc_step(h, keys, q_in, logp_in, grad_in, q_out, logp_out, grad_out, step_size, step_size_dev, L,
                               make_info(info));
-  if (use_big_path(h))
-    return bjx_big_hmc_step(h, keys, q_in, logp_in, grad_in, q_out, logp_out, grad_out, step_size, step_size_dev, L,
-                            make_info(info));
+    case ROUTE_ROWS: break;
+  }
   LaunchArgs a{};
   a.P = make_params(h, step_size, step_size_dev);
   a.keys = keys;
@@ -615,13 +593,13 @@ extern "C" int bjx_ghmc_step(bjx_handle_t h, const uint32_t* keys, float* q, flo
   const void* ptrs[] = {q, grad, p};
   int rc = check_ready(h, true, ptrs, 3);
   if (rc) return rc;
-  if (!keys || !logp || !slice) return fail(h, BJX_E_INVALID, "bad argument");
-  if (use_dense_path(h) || use_big_path(h))
-    return fail(h, BJX_E_UNSUPPORTED, "generalized HMC is built for dim <= 1024 (dense metrics: dim <= 128)");
+  if (!keys || !logp || !slice) return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  if (transition_route(h) != ROUTE_ROWS)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "generalized HMC is built for dim <= 1024 (dense metrics: dim <= 128)");
   if ((imm_rows != nullptr) != (msqrt_rows != nullptr) || chains_per_group < 1)
-    return fail(h, BJX_E_INVALID, "imm_rows and msqrt_rows come together; chains_per_group >= 1");
+    return bjx_fail(h, BJX_E_INVALID, "imm_rows and msqrt_rows come together; chains_per_group >= 1");
   if (imm_rows && (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK))
-    return fail(h, BJX_E_INVALID, "per-row momentum scales need a diagonal metric on the handle");
+    return bjx_fail(h, BJX_E_INVALID, "per-row momentum scales need a diagonal metric on the handle");
   LaunchArgs a{};
   a.P = make_params(h, step_size, step_size_dev);
   if (imm_rows) {  // MEADS: one inverse-mass row per fold (meads_adaptation.py:587-606)
@@ -650,11 +628,11 @@ extern "C" int bjx_mhmc_step(bjx_handle_t h, const uint32_t* keys, const float* 
   const void* ptrs[] = {q_in, grad_in, q_out, grad_out};
   int rc = check_ready(h, true, ptrs, 4);
   if (rc) return rc;
-  if (!keys || !logp_in || !logp_out || L < 1) return fail(h, BJX_E_INVALID, "bad argument");
-  if ((q_in == q_out) != (grad_in == grad_out) || (q_in == q_out) != (logp_in == logp_out))
-    return fail(h, BJX_E_INVALID, "in-place call must alias all of (q, logp, grad)");
-  if (use_dense_path(h) || h->sc == SC_BIG)
-    return fail(h, BJX_E_UNSUPPORTED, "multinomial HMC is built for dim <= 1024 (dense metrics: dim <= 128)");
+  if (!keys || !logp_in || !logp_out || L < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  rc = check_in_place(h, q_in, logp_in, grad_in, q_out, logp_out, grad_out);
+  if (rc) return rc;
+  if (transition_route(h) != ROUTE_ROWS)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "multinomial HMC is built for dim <= 1024 (dense metrics: dim <= 128)");
   LaunchArgs a{};
   a.P = make_params(h, step_size, step_size_dev);
   a.keys = keys;
@@ -665,6 +643,33 @@ extern "C" int bjx_mhmc_step(bjx_handle_t h, const uint32_t* keys, const float* 
   return dispatch(h, K_MHMC, true, a);
 }
 
+// ---- run loops ------------------------------------------------------------------------------------------
+// Step keys of a run loop: split(rng_key, num_steps) into h->sample_keys, on the device (util.py:203).
+static int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps) {
+  int rc = bjx_grow(h, h->sample_keys, h->sample_keys_cap, (size_t)num_steps, 2 * sizeof(uint32_t));
+  if (rc) return rc;
+  launch_prng_split(rng_key, 1, num_steps, h->sample_keys, h->stream);
+  BJX_CHECK_LAUNCH("k_prng_split");
+  return 0;
+}
+
+// For its lifetime every chain's key derives from one step key (bjx_set_key_mode 1); the caller's mode comes back after.
+struct SharedStepKeys {
+  bjx_handle_t h;
+  int saved;
+  explicit SharedStepKeys(bjx_handle_t h_) : h(h_), saved(h_->key_shared) { h->key_shared = 1; }
+  ~SharedStepKeys() { h->key_shared = saved; }
+};
+
+// history (optional) receives the positions after every `thin`-th transition: row (t + 1) / thin - 1 after transition t
+static int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q) {
+  if (!history || ((t + 1) % thin) != 0) return 0;
+  const size_t row = (size_t)h->cfg.n_chains * h->cfg.dim;
+  BJX_CUDA(cudaMemcpyAsync(history + (size_t)((t + 1) / thin - 1) * row, q, row * sizeof(float), cudaMemcpyDeviceToDevice,
+                           h->stream));
+  return 0;
+}
+
 // run_inference_algorithm (blackjax/util.py:150-213) for HMC / multinomial HMC, natively: keys = split(rng_key,
 // num_steps) (util.py:203) on the device, then num_steps transitions enqueued back to back with NO host
 // synchronisation; per-chain keys come from the step key inside the kernel (bjx_set_key_mode's chain_offset is
@@ -672,38 +677,24 @@ extern "C" int bjx_mhmc_step(bjx_handle_t h, const uint32_t* keys, const float* 
 extern "C" int bjx_hmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, float* grad, float step_size,
                               const float* step_size_dev, int32_t L, int32_t num_steps, int32_t multinomial,
                               float* history, int32_t thin, float* acceptance_history) {
-  if (!h || !rng_key || num_steps < 0 || thin < 1) return fail(h, BJX_E_INVALID, "bad argument");
+  if (!h || !rng_key || num_steps < 0 || thin < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  if ((size_t)num_steps > h->sample_keys_cap) {
-    if (h->sample_keys) BJX_CUDA(cudaFree(h->sample_keys));
-    h->sample_keys = nullptr;
-    BJX_CUDA(cudaMalloc((void**)&h->sample_keys, (size_t)num_steps * 2 * sizeof(uint32_t)));
-    h->sample_keys_cap = (size_t)num_steps;
-  }
-  launch_prng_split(rng_key, 1, num_steps, h->sample_keys, h->stream);
-  BJX_CHECK_LAUNCH("k_prng_split");
-  const int saved_mode = h->key_shared;
-  h->key_shared = 1;
-  const size_t row_bytes = (size_t)h->cfg.n_chains * h->cfg.dim * sizeof(float);
-  int rc = 0;
+  int rc = split_step_keys(h, rng_key, num_steps);
+  if (rc) return rc;
+  SharedStepKeys shared(h);
   for (int t = 0; t < num_steps && rc == 0; ++t) {
     bjx_info info{};
     info.acceptance_rate = acceptance_history ? acceptance_history + (size_t)t * h->cfg.n_chains : nullptr;
     const uint32_t* key_t = h->sample_keys + 2 * (size_t)t;
     rc = multinomial ? bjx_mhmc_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, L, &info)
                      : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, L, &info);
-    if (rc == 0 && history && ((t + 1) % thin) == 0) {
-      cudaError_t e = cudaMemcpyAsync(history + (size_t)((t + 1) / thin - 1) * h->cfg.n_chains * h->cfg.dim, q, row_bytes,
-                                      cudaMemcpyDeviceToDevice, h->stream);
-      if (e != cudaSuccess) rc = cuda_fail(h, e, "cudaMemcpyAsync(history)");
-    }
+    if (rc == 0) rc = copy_history(h, history, thin, t, q);
   }
-  h->key_shared = saved_mode;
   return rc;
 }
 
-// ---- NUTS workspace -------------------------------------------------------------------------------------
+// ---- NUTS ------------------------------------------------------------------------------------------------
 static int ensure_ws(bjx_handle_t h) {
   const int depth = h->cfg.max_tree_depth;
   if (h->ws_block && h->ws_depth == depth) return 0;
@@ -741,6 +732,35 @@ static int ensure_ws(bjx_handle_t h) {
 
 int bjx_ensure_nuts_ws(bjx_handle_t h) { return ensure_ws(h); }
 
+// Preamble of a NUTS run on `route` (bjx_nuts_step, bjx_nuts_sample's decoupled sampler), after the caller's argument
+// checks: the depth check and the route's rejections, then, on the row kernels, the workspace and cleared counters
+// (bjx_dense_nuts_step sets up its own).
+static int nuts_prepare(bjx_handle_t h, Route route, int max_num_doublings) {
+  if (max_num_doublings < 0 || max_num_doublings > h->cfg.max_tree_depth)
+    return bjx_fail(h, BJX_E_INVALID, "max_num_doublings exceeds the handle's max_tree_depth");
+  switch (route) {
+    case ROUTE_BIG: return bjx_fail(h, BJX_E_UNSUPPORTED, "NUTS is built for dim <= 1024");
+    case ROUTE_DENSE:
+      if (h->general_integrator) return bjx_fail(h, BJX_E_UNSUPPORTED, "only velocity Verlet is built for the tensor-core dense path");
+      return 0;
+    case ROUTE_ROWS: break;
+  }
+  int rc = ensure_ws(h);
+  if (rc) return rc;
+  BJX_CUDA(cudaMemsetAsync(h->ws.counters, 0, 64 * sizeof(int), h->stream));
+  return 0;
+}
+
+// Whether the row kernels keep the checkpoints of `depth` doublings in shared memory, next to the row the dense-metric,
+// dense-target and plug-in kernels keep there: only under the 48 KB default dynamic-smem limit.
+static int ckpt_in_smem(bjx_handle_t h, int depth) {
+  const size_t ckpt_bytes = sizeof(float) * kWarpsPerBlock * 2 * (size_t)depth * h->cfg.dim;
+  const size_t dm_bytes = (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK ||
+                           h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN || h->cfg.target.kind == BJX_TARGET_USER)
+                              ? sizeof(float) * kWarpsPerBlock * h->cfg.dim : 0;
+  return (ckpt_bytes + dm_bytes <= 40 * 1024) ? 1 : 0;
+}
+
 extern "C" int bjx_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in,
                              const float* grad_in, float* q_out, float* logp_out, float* grad_out, float step_size,
                              const float* step_size_dev, int32_t max_num_doublings, const bjx_info* info,
@@ -748,17 +768,15 @@ extern "C" int bjx_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* 
   const void* ptrs[] = {q_in, grad_in, q_out, grad_out};
   int rc = check_ready(h, true, ptrs, 4);
   if (rc) return rc;
-  if (!logp_in || !logp_out) return fail(h, BJX_E_INVALID, "null array argument");
+  if (!logp_in || !logp_out) return bjx_fail(h, BJX_E_INVALID, "null array argument");
   if ((momentum_override == nullptr) != (key_integrator_override == nullptr))
-    return fail(h, BJX_E_INVALID, "momentum_override and key_integrator_override go together");
-  if (!keys && !key_integrator_override) return fail(h, BJX_E_INVALID, "null keys");
-  if (max_num_doublings < 0 || max_num_doublings > h->cfg.max_tree_depth)
-    return fail(h, BJX_E_INVALID, "max_num_doublings exceeds the handle's max_tree_depth");
-  if ((q_in == q_out) != (grad_in == grad_out) || (q_in == q_out) != (logp_in == logp_out))
-    return fail(h, BJX_E_INVALID, "in-place call must alias all of (q, logp, grad)");
-  if (h->sc == SC_BIG && !use_dense_path(h)) return fail(h, BJX_E_UNSUPPORTED, "NUTS is built for dim <= 1024");
-  if (use_dense_path(h) && h->general_integrator)
-    return fail(h, BJX_E_UNSUPPORTED, "only velocity Verlet is built for the tensor-core dense path");
+    return bjx_fail(h, BJX_E_INVALID, "momentum_override and key_integrator_override go together");
+  if (!keys && !key_integrator_override) return bjx_fail(h, BJX_E_INVALID, "null keys");
+  rc = check_in_place(h, q_in, logp_in, grad_in, q_out, logp_out, grad_out);
+  if (rc) return rc;
+  const Route route = transition_route(h);
+  rc = nuts_prepare(h, route, max_num_doublings);
+  if (rc) return rc;
   auto endpoint_info = [&]() -> int {
     if (info) {
       const size_t bytes = (size_t)h->cfg.n_chains * h->cfg.dim * sizeof(float);
@@ -769,15 +787,12 @@ extern "C" int bjx_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* 
     }
     return 0;
   };
-  if (use_dense_path(h)) {  // dense metric / dense target beyond 128 dims: lock-step leaves on the tensor-core products
+  if (route == ROUTE_DENSE) {  // dense metric / dense target beyond 128 dims: lock-step leaves on the tensor-core products
     rc = bjx_dense_nuts_step(h, keys, q_in, logp_in, grad_in, q_out, logp_out, grad_out, step_size, step_size_dev,
                              max_num_doublings, make_info(info), momentum_override, key_integrator_override);
     return rc ? rc : endpoint_info();
   }
-  rc = ensure_ws(h);
-  if (rc) return rc;
   const int C = h->cfg.n_chains;
-  BJX_CUDA(cudaMemsetAsync(h->ws.counters, 0, 64 * sizeof(int), h->stream));
 
   LaunchArgs a{};
   a.P = make_params(h, step_size, step_size_dev);
@@ -799,11 +814,7 @@ extern "C" int bjx_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* 
   // counters[launch]: a fixed grid strides over the list, so a doubling that nobody needs costs one empty launch.
   // Chains never interact, so nothing forces them through the tree in lock step.
   const int kFusedDoublings = 4;  // (the kernel's lane-parallel key schedule handles up to 10 doublings per launch)
-  const size_t ckpt_bytes = sizeof(float) * kWarpsPerBlock * 2 * (size_t)h->cfg.max_tree_depth * h->cfg.dim;
-  const size_t dm_bytes = (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK ||
-                           h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN || h->cfg.target.kind == BJX_TARGET_USER)
-                              ? sizeof(float) * kWarpsPerBlock * h->cfg.dim : 0;
-  a.ckpt_smem = (ckpt_bytes + dm_bytes <= 40 * 1024) ? 1 : 0;  // stay under the 48 KB default dynamic-smem limit
+  a.ckpt_smem = ckpt_in_smem(h, h->cfg.max_tree_depth);
   int64_t launches = 0;
   const int d_fused = max_num_doublings < kFusedDoublings ? max_num_doublings : kFusedDoublings;
   if (max_num_doublings > 0) {
@@ -840,7 +851,7 @@ extern "C" int bjx_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* 
 }
 
 extern "C" int bjx_nuts_last_stats(bjx_handle_t h, int64_t* leaf_launches, int64_t* depth_reached) {
-  if (!h) return fail(h, BJX_E_INVALID, "null handle");
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
   if (leaf_launches) *leaf_launches = h->last_leaf_launches;
   if (depth_reached) {
     if (h->last_depth < 0 && h->ws_block) {  // the one host round trip of the NUTS path, and only on request
@@ -859,61 +870,42 @@ extern "C" int bjx_nuts_last_stats(bjx_handle_t h, int64_t* leaf_launches, int64
 extern "C" int bjx_nuts_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, float* grad, float step_size,
                                const float* step_size_dev, int32_t max_num_doublings, int32_t num_steps, float* history,
                                int32_t thin, float* acceptance_history, int32_t* num_integration_steps_history) {
-  if (!h || !rng_key || num_steps < 0 || thin < 1) return fail(h, BJX_E_INVALID, "bad argument");
+  if (!h || !rng_key || num_steps < 0 || thin < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  if ((size_t)num_steps > h->sample_keys_cap) {
-    if (h->sample_keys) BJX_CUDA(cudaFree(h->sample_keys));
-    h->sample_keys = nullptr;
-    BJX_CUDA(cudaMalloc((void**)&h->sample_keys, (size_t)num_steps * 2 * sizeof(uint32_t)));
-    h->sample_keys_cap = (size_t)num_steps;
-  }
-  launch_prng_split(rng_key, 1, num_steps, h->sample_keys, h->stream);
-  BJX_CHECK_LAUNCH("k_prng_split");
-  const int saved_mode = h->key_shared;
-  h->key_shared = 1;
-  const size_t C = h->cfg.n_chains, row_bytes = C * h->cfg.dim * sizeof(float);
-  int rc = 0;
+  int rc = split_step_keys(h, rng_key, num_steps);
+  if (rc) return rc;
+  SharedStepKeys shared(h);
+  const size_t C = h->cfg.n_chains;
   // Enough transitions to amortise the ragged end: the chains run decoupled, every warp taking whole chains through all
   // num_steps transitions (k_nuts_chains).  BJX_NUTS_DECOUPLED=0 keeps the step-synchronous loop (same results).
   static const bool decoupled_ok = [] { const char* e = getenv("BJX_NUTS_DECOUPLED"); return !(e && e[0] == '0'); }();
-  if (decoupled_ok && num_steps >= 4 && max_num_doublings > 0 && !use_dense_path(h)) {  // (the dense path is lock step)
+  const Route route = transition_route(h);
+  if (decoupled_ok && num_steps >= 4 && max_num_doublings > 0 && route != ROUTE_DENSE) {  // (the dense path is lock step)
     const void* ptrs[] = {q, grad};
     rc = check_ready(h, true, ptrs, 2);
-    if (rc == 0 && !logp) rc = fail(h, BJX_E_INVALID, "null array argument");
-    if (rc == 0 && max_num_doublings > h->cfg.max_tree_depth)
-      rc = fail(h, BJX_E_INVALID, "max_num_doublings exceeds the handle's max_tree_depth");
-    if (rc == 0 && h->sc == SC_BIG) rc = fail(h, BJX_E_UNSUPPORTED, "NUTS is built for dim <= 1024");
-    if (rc == 0) rc = ensure_ws(h);
-    if (rc == 0) {
-      cudaError_t e = cudaMemsetAsync(h->ws.counters, 0, 64 * sizeof(int), h->stream);
-      if (e != cudaSuccess) rc = cuda_fail(h, e, "cudaMemsetAsync(counters)");
-    }
-    if (rc == 0) {
-      LaunchArgs a{};
-      a.P = make_params(h, step_size, step_size_dev);
-      a.ws = h->ws;
-      a.q_out = q; a.logp_out = logp; a.g_out = grad;
-      const size_t ckpt_bytes = sizeof(float) * kWarpsPerBlock * 2 * (size_t)max_num_doublings * h->cfg.dim;
-      const size_t dm_bytes = (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK ||
-                               h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN || h->cfg.target.kind == BJX_TARGET_USER)
-                                  ? sizeof(float) * kWarpsPerBlock * h->cfg.dim : 0;
-      a.sample.step_keys = h->sample_keys;
-      a.sample.num_steps = num_steps;
-      a.sample.max_doublings = max_num_doublings;
-      a.sample.ckpt_smem = (ckpt_bytes + dm_bytes <= 40 * 1024) ? 1 : 0;
-      a.sample.history = history;
-      a.sample.thin = thin;
-      a.sample.acceptance_history = acceptance_history;
-      a.sample.nint_history = num_integration_steps_history;
-      a.sample.leapfrogs = nullptr;
-      a.sample.queue = h->ws.counters + 62;
-      a.grid_override = sm_count();  // the launcher multiplies by the CTAs that stay resident per SM
-      rc = dispatch(h, K_NUTS_CHAINS, true, a);
-      h->last_leaf_launches = 1;
-      h->last_depth = -1;
-    }
-    h->key_shared = saved_mode;
+    if (rc) return rc;
+    if (!logp) return bjx_fail(h, BJX_E_INVALID, "null array argument");
+    rc = nuts_prepare(h, route, max_num_doublings);
+    if (rc) return rc;
+    LaunchArgs a{};
+    a.P = make_params(h, step_size, step_size_dev);
+    a.ws = h->ws;
+    a.q_out = q; a.logp_out = logp; a.g_out = grad;
+    a.sample.step_keys = h->sample_keys;
+    a.sample.num_steps = num_steps;
+    a.sample.max_doublings = max_num_doublings;
+    a.sample.ckpt_smem = ckpt_in_smem(h, max_num_doublings);
+    a.sample.history = history;
+    a.sample.thin = thin;
+    a.sample.acceptance_history = acceptance_history;
+    a.sample.nint_history = num_integration_steps_history;
+    a.sample.leapfrogs = nullptr;
+    a.sample.queue = h->ws.counters + 62;
+    a.grid_override = sm_count();  // the launcher multiplies by the CTAs that stay resident per SM
+    rc = dispatch(h, K_NUTS_CHAINS, true, a);
+    h->last_leaf_launches = 1;
+    h->last_depth = -1;
     return rc;
   }
   for (int t = 0; t < num_steps && rc == 0; ++t) {
@@ -922,13 +914,8 @@ extern "C" int bjx_nuts_sample(bjx_handle_t h, const uint32_t* rng_key, float* q
     info.num_integration_steps = num_integration_steps_history ? num_integration_steps_history + (size_t)t * C : nullptr;
     rc = bjx_nuts_step(h, h->sample_keys + 2 * (size_t)t, q, logp, grad, q, logp, grad, step_size, step_size_dev,
                        max_num_doublings, &info, nullptr, nullptr);
-    if (rc == 0 && history && ((t + 1) % thin) == 0) {
-      cudaError_t e = cudaMemcpyAsync(history + (size_t)((t + 1) / thin - 1) * C * h->cfg.dim, q, row_bytes,
-                                      cudaMemcpyDeviceToDevice, h->stream);
-      if (e != cudaSuccess) rc = cuda_fail(h, e, "cudaMemcpyAsync(history)");
-    }
+    if (rc == 0) rc = copy_history(h, history, thin, t, q);
   }
-  h->key_shared = saved_mode;
   return rc;
 }
 
@@ -949,22 +936,14 @@ extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_r
                                     int32_t max_num_doublings, int32_t num_integration_steps, float* eps_history,
                                     float* acceptance_scratch, int32_t* steps_scratch, unsigned long long* leapfrog_counter) {
   if (!h || !rng_key || !schedule || !q || !logp || !grad || !state || !step_size_chain || !imm || !acceptance_scratch || num_steps < 0)
-    return fail(h, BJX_E_INVALID, "bad argument");
+    return bjx_fail(h, BJX_E_INVALID, "bad argument");
   if ((max_num_doublings > 0) == (num_integration_steps > 0))
-    return fail(h, BJX_E_INVALID, "give max_num_doublings (NUTS) or num_integration_steps (HMC)");
+    return bjx_fail(h, BJX_E_INVALID, "give max_num_doublings (NUTS) or num_integration_steps (HMC)");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  if ((size_t)num_steps > h->sample_keys_cap) {
-    if (h->sample_keys) BJX_CUDA(cudaFree(h->sample_keys));
-    h->sample_keys = nullptr;
-    BJX_CUDA(cudaMalloc((void**)&h->sample_keys, (size_t)num_steps * 2 * sizeof(uint32_t)));
-    h->sample_keys_cap = (size_t)num_steps;
-  }
-  launch_prng_split(rng_key, 1, num_steps, h->sample_keys, h->stream);
-  BJX_CHECK_LAUNCH("k_prng_split");
-  const int saved_mode = h->key_shared;
-  h->key_shared = 1;
-  int rc = 0;
+  int rc = split_step_keys(h, rng_key, num_steps);
+  if (rc) return rc;
+  SharedStepKeys shared(h);
   for (int t = 0; t < num_steps && rc == 0; ++t) {
     bjx_info info{};
     info.acceptance_rate = acceptance_scratch;
@@ -981,7 +960,6 @@ extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_r
       rc = bjx_adapt_shared_update(h, nccl_comm, n_ranks, state, q, acceptance_scratch, schedule[t] & 1, (schedule[t] >> 1) & 1,
                                    target_acceptance, step_size_chain, imm, eps_history);
   }
-  h->key_shared = saved_mode;
   return rc;
 }
 
@@ -994,13 +972,13 @@ extern "C" int bjx_set_default_stream(void* stream) {
   return 0;
 }
 #define BJX_PRNG_PROLOGUE()                                                        \
-  if (!keys || !out || n_keys < 0) return fail(h, BJX_E_INVALID, "bad argument");  \
+  if (!keys || !out || n_keys < 0) return bjx_fail(h, BJX_E_INVALID, "bad argument");  \
   if (h) BJX_CUDA(cudaSetDevice(h->cfg.device));                                   \
   cudaStream_t pstream = h ? h->stream : t_default_stream;
 
 extern "C" int bjx_prng_split(bjx_handle_t h, const uint32_t* keys, int64_t n_keys, int32_t num, uint32_t* out) {
   BJX_PRNG_PROLOGUE();
-  if (num < 0) return fail(h, BJX_E_INVALID, "bad argument");
+  if (num < 0) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   launch_prng_split(keys, n_keys, num, out, pstream);
   BJX_CHECK_LAUNCH("k_prng_split");
   return 0;
@@ -1013,14 +991,14 @@ extern "C" int bjx_prng_fold_in(bjx_handle_t h, const uint32_t* keys, int64_t n_
 }
 extern "C" int bjx_prng_random_bits(bjx_handle_t h, const uint32_t* keys, int64_t n_keys, int64_t per_key, uint32_t* out) {
   BJX_PRNG_PROLOGUE();
-  if (per_key < 0 || per_key > 0xFFFFFFFFll) return fail(h, BJX_E_INVALID, "bad per_key");
+  if (per_key < 0 || per_key > 0xFFFFFFFFll) return bjx_fail(h, BJX_E_INVALID, "bad per_key");
   launch_prng_draw(0, keys, n_keys, per_key, out, pstream);
   BJX_CHECK_LAUNCH("k_prng_draw");
   return 0;
 }
 extern "C" int bjx_prng_uniform(bjx_handle_t h, const uint32_t* keys, int64_t n_keys, int64_t per_key, float* out) {
   BJX_PRNG_PROLOGUE();
-  if (per_key < 0 || per_key > 0xFFFFFFFFll) return fail(h, BJX_E_INVALID, "bad per_key");
+  if (per_key < 0 || per_key > 0xFFFFFFFFll) return bjx_fail(h, BJX_E_INVALID, "bad per_key");
   launch_prng_draw(1, keys, n_keys, per_key, out, pstream);
   BJX_CHECK_LAUNCH("k_prng_draw");
   return 0;
@@ -1030,14 +1008,14 @@ extern "C" int bjx_prng_uniform(bjx_handle_t h, const uint32_t* keys, int64_t n_
 extern "C" int bjx_prng_randint(bjx_handle_t h, const uint32_t* keys, int64_t n_keys, int64_t per_key, int32_t minval,
                                 int32_t maxval, int32_t* out) {
   BJX_PRNG_PROLOGUE();
-  if (per_key < 0 || per_key > 0xFFFFFFFFll) return fail(h, BJX_E_INVALID, "bad per_key");
+  if (per_key < 0 || per_key > 0xFFFFFFFFll) return bjx_fail(h, BJX_E_INVALID, "bad per_key");
   launch_prng_randint(keys, n_keys, per_key, minval, maxval, out, pstream);
   BJX_CHECK_LAUNCH("k_prng_randint");
   return 0;
 }
 extern "C" int bjx_prng_normal(bjx_handle_t h, const uint32_t* keys, int64_t n_keys, int64_t per_key, float* out) {
   BJX_PRNG_PROLOGUE();
-  if (per_key < 0 || per_key > 0xFFFFFFFFll) return fail(h, BJX_E_INVALID, "bad per_key");
+  if (per_key < 0 || per_key > 0xFFFFFFFFll) return bjx_fail(h, BJX_E_INVALID, "bad per_key");
   launch_prng_draw(2, keys, n_keys, per_key, out, pstream);
   BJX_CHECK_LAUNCH("k_prng_draw");
   return 0;
@@ -1045,63 +1023,63 @@ extern "C" int bjx_prng_normal(bjx_handle_t h, const uint32_t* keys, int64_t n_k
 
 // ---- window adaptation ------------------------------------------------------------------------------------
 extern "C" int bjx_da_init(bjx_handle_t h, float* st, const float* eps0, float* eps_out) {
-  if (!h || !st || !eps0) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !st || !eps0) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_da(0, h->cfg.n_chains, st, eps0, 0.f, eps_out, h->stream);
   BJX_CHECK_LAUNCH("k_da_init");
   return 0;
 }
 extern "C" int bjx_da_update(bjx_handle_t h, float* st, const float* acc, float target, float* eps_out) {
-  if (!h || !st || !acc) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !st || !acc) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_da(1, h->cfg.n_chains, st, acc, target, eps_out, h->stream);
   BJX_CHECK_LAUNCH("k_da_update");
   return 0;
 }
 extern "C" int bjx_da_reset(bjx_handle_t h, float* st, float* eps_out) {
-  if (!h || !st) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !st) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_da(2, h->cfg.n_chains, st, nullptr, 0.f, eps_out, h->stream);
   BJX_CHECK_LAUNCH("k_da_reset");
   return 0;
 }
 extern "C" int bjx_da_final(bjx_handle_t h, const float* st, float* eps_out) {
-  if (!h || !st || !eps_out) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !st || !eps_out) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_da(3, h->cfg.n_chains, const_cast<float*>(st), nullptr, 0.f, eps_out, h->stream);
   BJX_CHECK_LAUNCH("k_da_final");
   return 0;
 }
 extern "C" int bjx_welford_update(bjx_handle_t h, const float* q, float* mean, float* m2, int32_t new_count) {
-  if (!h || !q || !mean || !m2 || new_count < 1) return fail(h, BJX_E_INVALID, "bad argument");
+  if (!h || !q || !mean || !m2 || new_count < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_welford_update((long long)h->cfg.n_chains * h->cfg.dim, q, mean, m2, new_count, h->stream);
   BJX_CHECK_LAUNCH("k_welford_update");
   return 0;
 }
 extern "C" int bjx_welford_final(bjx_handle_t h, float* mean, float* m2, int32_t count, float* imm_out) {
-  if (!h || !mean || !m2 || !imm_out || count < 2) return fail(h, BJX_E_INVALID, "bad argument");
+  if (!h || !mean || !m2 || !imm_out || count < 2) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_welford_final((long long)h->cfg.n_chains * h->cfg.dim, mean, m2, count, imm_out, h->stream);
   BJX_CHECK_LAUNCH("k_welford_final");
   return 0;
 }
 extern "C" int bjx_welford_dense_update(bjx_handle_t h, const float* q, float* mean, float* m2, int32_t new_count) {
-  if (!h || !q || !mean || !m2 || new_count < 1) return fail(h, BJX_E_INVALID, "bad argument");
+  if (!h || !q || !mean || !m2 || new_count < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_welford_dense_update(h->cfg.n_chains, h->cfg.dim, q, mean, m2, new_count, h->stream);
   BJX_CHECK_LAUNCH("k_welford_dense_m2");
   return 0;
 }
 extern "C" int bjx_welford_dense_final(bjx_handle_t h, float* mean, float* m2, int32_t count, float* imm_out) {
-  if (!h || !mean || !m2 || !imm_out || count < 2) return fail(h, BJX_E_INVALID, "bad argument");
+  if (!h || !mean || !m2 || !imm_out || count < 2) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_welford_dense_final(h->cfg.n_chains, h->cfg.dim, mean, m2, count, imm_out, h->stream);
   BJX_CHECK_LAUNCH("k_welford_dense_final");
   return 0;
 }
 extern "C" int bjx_pooled_stats(bjx_handle_t h, const float* q, const float* acc, float* out) {
-  if (!h || !q || !acc || !out) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !q || !acc || !out) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_pooled_stats(h->cfg.n_chains, h->cfg.dim, q, acc, out, h->stream);
   BJX_CHECK_LAUNCH("k_pooled_stats");
@@ -1109,15 +1087,11 @@ extern "C" int bjx_pooled_stats(bjx_handle_t h, const float* q, const float* acc
 }
 
 extern "C" int bjx_pooled_stats_dense(bjx_handle_t h, const float* q, const float* acc, float* out) {
-  if (!h || !q || !acc || !out) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !q || !acc || !out) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   const size_t need = pooled_dense_scratch_floats(h->cfg.dim) * sizeof(float);
-  if (h->pool_scratch_bytes < need) {
-    if (h->pool_scratch) BJX_CUDA(cudaFree(h->pool_scratch));
-    h->pool_scratch = nullptr;
-    BJX_CUDA(cudaMalloc((void**)&h->pool_scratch, need));
-    h->pool_scratch_bytes = need;
-  }
+  int rc = bjx_grow(h, h->pool_scratch, h->pool_scratch_bytes, need, 1);
+  if (rc) return rc;
   launch_pooled_stats_dense(h->cfg.n_chains, h->cfg.dim, q, acc, out, h->pool_scratch, h->stream);
   BJX_CHECK_LAUNCH("k_pooled_stats_dense");
   return 0;
@@ -1127,9 +1101,9 @@ extern "C" int bjx_pooled_stats_dense(bjx_handle_t h, const float* q, const floa
 // axis 0): rhat_out [D].  scratch: device buffer of at least 2*C*D + 4 + 4*D floats.
 extern "C" int bjx_potential_scale_reduction(bjx_handle_t h, const float* history, int32_t num_samples, float* rhat_out,
                                              float* scratch) {
-  if (!h || !history || !rhat_out || !scratch) return fail(h, BJX_E_INVALID, "null argument");
+  if (!h || !history || !rhat_out || !scratch) return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (num_samples < 2 || h->cfg.n_chains < 2)
-    return fail(h, BJX_E_INVALID, "potential_scale_reduction as implemented only works for two or more chains (and draws)");
+    return bjx_fail(h, BJX_E_INVALID, "potential_scale_reduction as implemented only works for two or more chains (and draws)");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_rhat(num_samples, h->cfg.n_chains, h->cfg.dim, history, rhat_out, scratch, h->stream);
   BJX_CHECK_LAUNCH("k_rhat");
@@ -1143,9 +1117,9 @@ extern "C" int64_t bjx_ess_scratch_floats(int32_t num_samples, int32_t n_chains,
 }
 extern "C" int bjx_effective_sample_size(bjx_handle_t h, const float* history, int32_t num_samples, float* ess_out,
                                          float* scratch) {
-  if (!h || !history || !ess_out || !scratch) return fail(h, BJX_E_INVALID, "null argument");
-  if (num_samples < 2) return fail(h, BJX_E_INVALID, "The input array must have at least 2 samples");
-  if ((reinterpret_cast<uintptr_t>(scratch) & 7u) != 0) return fail(h, BJX_E_INVALID, "scratch must be 8-byte aligned");
+  if (!h || !history || !ess_out || !scratch) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (num_samples < 2) return bjx_fail(h, BJX_E_INVALID, "The input array must have at least 2 samples");
+  if ((reinterpret_cast<uintptr_t>(scratch) & 7u) != 0) return bjx_fail(h, BJX_E_INVALID, "scratch must be 8-byte aligned");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   launch_ess(num_samples, h->cfg.n_chains, h->cfg.dim, history, ess_out, scratch, h->stream);
   BJX_CHECK_LAUNCH("k_ess");

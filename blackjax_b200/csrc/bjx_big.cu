@@ -9,8 +9,6 @@
 // Same reference functions as the warp kernels: hmc.py:90-92 (init), metrics.py:260-270 (momentum draw,
 // kinetic energy), integrators.py:104-150 (velocity Verlet), hmc.py:279-312 (transition),
 // proposal.py:45-48,214-235 (accept).  Diagonal metrics only; NUTS is not built for this size class.
-#include <stdlib.h>
-
 #include "bjx_handle.h"
 #include "bjx_internal.h"
 #include "bjx_big.cuh"
@@ -285,12 +283,6 @@ __global__ void __launch_bounds__(T) k_big2_hmc_hier(BigParams P, const uint32_t
 }
 }  // namespace bjx
 
-#define BG_LAUNCH(where)                                           \
-  do {                                                             \
-    cudaError_t e_ = cudaGetLastError();                           \
-    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, where);     \
-  } while (0)
-
 static BigParams big_params(bjx_handle_t h, float eps, const float* eps_dev) {
   BigParams P;
   P.C = h->cfg.n_chains;
@@ -314,25 +306,6 @@ static BigParams big_params(bjx_handle_t h, float eps, const float* eps_dev) {
   P.chain_offset = h->chain_offset;
   return P;
 }
-
-// threads per CTA of the two-chains-per-CTA hierarchical-logit kernel (BJX_BIG2_THREADS = 512 | 768; 0 = one chain per CTA)
-static int big2_threads() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("BJX_BIG2_THREADS");
-    v = e ? atoi(e) : 512;
-    if (v != 0 && v != 512 && v != 768) v = 512;
-  }
-  return v;
-}
-
-template <class K>
-static int big_smem(bjx_handle_t h, K kernel, size_t bytes) {
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  if (e != cudaSuccess) return bjx_cuda_fail(h, e, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize)");
-  return 0;
-}
-
 
 static int big_dispatch(bjx_handle_t h, int kernel_id, BigLaunchArgs& a) {
   a.stream = h->stream;
@@ -363,13 +336,13 @@ int bjx_big_init_state(bjx_handle_t h, const float* q, float* logp_out, float* g
 int bjx_big_sample_momentum(bjx_handle_t h, const uint32_t* keys, float* p_out) {
   BigParams P = big_params(h, 0.f, nullptr);
   k_big_momentum<<<h->cfg.n_chains, kBigThreads, 0, h->stream>>>(P, keys, p_out);
-  BG_LAUNCH("k_big_momentum");
+  BJX_CHECK_LAUNCH("k_big_momentum");
   return 0;
 }
 int bjx_big_energy(bjx_handle_t h, const float* p, const float* logp, float* e_out) {
   BigParams P = big_params(h, 0.f, nullptr);
   k_big_energy<<<h->cfg.n_chains, kBigThreads, 0, h->stream>>>(P, p, logp, e_out);
-  BG_LAUNCH("k_big_energy");
+  BJX_CHECK_LAUNCH("k_big_energy");
   return 0;
 }
 int bjx_big_leapfrog(bjx_handle_t h, float* q, float* p, float* logp, float* g, float eps, const float* eps_dev, int n) {
@@ -382,19 +355,13 @@ int bjx_big_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
                      float* q_out, float* logp_out, float* g_out, float eps, const float* eps_dev, int L,
                      const InfoPtrs& info) {
   BigParams P = big_params(h, eps, eps_dev);
-  if (h->cfg.target.kind == BJX_TARGET_HIER_LOGIT && h->cfg.dim <= 10240 && big2_threads() > 0) {
-    // two chains per CTA, momentum in registers (see k_big2_hmc_hier)
+  if (h->cfg.target.kind == BJX_TARGET_HIER_LOGIT && h->cfg.dim <= 10240) {
+    // two chains per CTA, momentum in registers (see k_big2_hmc_hier); rows beyond 10240 run one chain per CTA
     const size_t smem = (4 * (size_t)h->cfg.dim + 10 * 32) * sizeof(float);
     const int ctas = (h->cfg.n_chains + 1) / 2;
-    int rc;
-    if (big2_threads() == 512) {
-      if ((rc = big_smem(h, k_big2_hmc_hier<512>, smem))) return rc;
-      k_big2_hmc_hier<512><<<ctas, 512, smem, h->stream>>>(P, keys, q_in, logp_in, g_in, q_out, logp_out, g_out, L, info);
-    } else {
-      if ((rc = big_smem(h, k_big2_hmc_hier<768>, smem))) return rc;
-      k_big2_hmc_hier<768><<<ctas, 768, smem, h->stream>>>(P, keys, q_in, logp_in, g_in, q_out, logp_out, g_out, L, info);
-    }
-    BG_LAUNCH("k_big2_hmc_hier");
+    BJX_CUDA(cudaFuncSetAttribute(k_big2_hmc_hier<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_big2_hmc_hier<512><<<ctas, 512, smem, h->stream>>>(P, keys, q_in, logp_in, g_in, q_out, logp_out, g_out, L, info);
+    BJX_CHECK_LAUNCH("k_big2_hmc_hier");
     return 0;
   }
   BigLaunchArgs a{};

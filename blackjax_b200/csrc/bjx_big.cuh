@@ -5,6 +5,7 @@
 #pragma once
 #include "../../include/bjx.h"
 #include "bjx_kernels.cuh"
+#include "bjx_launch.cuh"  // (LaunchArgs: part of the plug-in ABI number)
 
 namespace bjx_user {
 struct BigModel;  // defined by a big-row plug-in's source
@@ -366,6 +367,10 @@ struct BigLaunchArgs {
   InfoPtrs info;
   cudaStream_t stream;
 };
+
+// What a target plug-in must have been built against (bjx_plugin_abi, bjx_plugin_built_for_abi): the C ABI version and
+// the layout of both launch-argument structs.
+inline int plugin_abi() { return BJX_VERSION * 100000 + (int)sizeof(LaunchArgs) + 7 * (int)sizeof(BigLaunchArgs); }
 
 // returns 0 or the cudaError_t of the attribute call / launch
 template <int TK>

@@ -323,17 +323,6 @@ __global__ void k_rows_accept(int C, int D, const uint32_t* __restrict__ keys, c
 }
 }  // namespace bjx
 
-#define DN_CUDA(call)                                                \
-  do {                                                               \
-    cudaError_t e_ = (call);                                         \
-    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, #call);       \
-  } while (0)
-#define DN_LAUNCH(where)                                             \
-  do {                                                               \
-    cudaError_t e_ = cudaGetLastError();                             \
-    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, where);       \
-  } while (0)
-
 static inline dim3 g4(long long n4) { return dim3((unsigned)((n4 + 255) / 256)); }
 static inline dim3 grow(int C) { return dim3((C + kRowWarps - 1) / kRowWarps); }
 
@@ -348,16 +337,8 @@ struct DenseWs {
 enum { MAT_IMM = 0, MAT_MSQRT = 1, MAT_PREC = 2 };
 enum { PL_P = 0, PL_Q = 1 };
 
-// The chain batch can be processed as kParts independent slices on separate streams (chains never interact, so the
-// slices share nothing but the constant matrices).  Slices fork from and join back into the handle's stream with
-// events.  With the operand split fused into the product's epilogue the loop is one persistent tensor-core kernel
-// after another, so one slice is the default.
-constexpr int kParts = 1;
-struct Part {
-  int c0, n;          // chains [c0, c0 + n)
-  cudaStream_t st;
-  int index;
-};
+// Every helper below works on the first n rows of its [C, D] / [C] arrays, all on the handle's stream: n = C, except for
+// NUTS (bjx_dense_nuts.cuh), whose leaves run on the chains still expanding, compacted into the first n rows.
 
 static int dense_ws(bjx_handle_t h, DenseWs& w) {
   const size_t C = h->cfg.n_chains, D = h->cfg.dim;
@@ -366,21 +347,8 @@ static int dense_ws(bjx_handle_t h, DenseWs& w) {
   const size_t xsb = ((C * 2 * KP * sizeof(uint16_t)) + 255) & ~(size_t)255;
   const size_t mat = ((D * 2 * KP * sizeof(uint16_t)) + 255) & ~(size_t)255;
   const size_t need = 4 * row + 11 * vec + 2 * xsb + 3 * mat + 256;
-  if (h->dense_bytes < need) {
-    if (h->dense_block) DN_CUDA(cudaFree(h->dense_block));
-    h->dense_block = nullptr;
-    DN_CUDA(cudaMalloc((void**)&h->dense_block, need));
-    h->dense_bytes = need;
-  }
-  if (!h->dense_streams_ready) {
-    for (int k = 0; k < 2; ++k) {
-      DN_CUDA(cudaStreamCreateWithFlags(&h->dense_stream[k], cudaStreamNonBlocking));
-      DN_CUDA(cudaEventCreateWithFlags(&h->dense_join[k], cudaEventDisableTiming));
-    }
-    DN_CUDA(cudaEventCreateWithFlags(&h->dense_fork, cudaEventDisableTiming));
-    DN_CUDA(cudaEventCreateWithFlags(&h->dense_stagger, cudaEventDisableTiming));
-    h->dense_streams_ready = true;
-  }
+  int rc = bjx_grow(h, h->dense_block, h->dense_bytes, need, 1);
+  if (rc) return rc;
   char* b = (char*)h->dense_block;
   w.p = (float*)b; w.v = (float*)(b + row); w.q = (float*)(b + 2 * row); w.g = (float*)(b + 3 * row);
   char* vb = b + 4 * row;
@@ -393,7 +361,7 @@ static int dense_ws(bjx_handle_t h, DenseWs& w) {
   w.mat_max = (float*)(xb + 2 * xsb + 3 * mat);
   w.mat_unscale = w.mat_max + 4;
   if (h->dense_bytes_built != need) {  // fresh block: zero the plane pads, every split matrix must be rebuilt
-    DN_CUDA(cudaMemsetAsync(vb, 0, 11 * vec + 2 * xsb + 3 * mat, h->stream));
+    BJX_CUDA(cudaMemsetAsync(vb, 0, 11 * vec + 2 * xsb + 3 * mat, h->stream));
     for (int m = 0; m < 3; ++m) h->dense_mat_src[m] = nullptr;
     h->dense_bytes_built = need;
   }
@@ -403,39 +371,17 @@ static int dense_ws(bjx_handle_t h, DenseWs& w) {
                          h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN ? h->cfg.target.precision : nullptr};
   for (int m = 0; m < 3; ++m) {
     if (src[m] && (h->dense_mat_src[m] != src[m] || h->dense_mat_ver[m] != h->dense_version)) {
-      DN_CUDA(cudaMemsetAsync(w.mat_max + m, 0, sizeof(float), h->stream));
+      BJX_CUDA(cudaMemsetAsync(w.mat_max + m, 0, sizeof(float), h->stream));
       k_absmax<<<sm_count(), 256, 0, h->stream>>>((long long)D * D / 4, src[m], w.mat_max + m);
-      DN_LAUNCH("k_absmax");
+      BJX_CHECK_LAUNCH("k_absmax");
       k_matrix_split2<<<g4((long long)D * D / 4), 256, 0, h->stream>>>((long long)D, (int)D, src[m], h->dense_mat_s[m],
                                                                       w.mat_max + m, w.mat_unscale + m);
-      DN_LAUNCH("k_matrix_split2");
+      BJX_CHECK_LAUNCH("k_matrix_split2");
       h->dense_mat_src[m] = src[m];
       h->dense_mat_ver[m] = h->dense_version;
     }
   }
   return 0;
-}
-
-// Run fn(part) for every slice: fork from the handle's stream, one stream per slice, join back.
-template <class F>
-static int for_parts(bjx_handle_t h, F fn) {
-  const int C = h->cfg.n_chains;
-  const int parts = (C >= 8192) ? kParts : 1;
-  if (parts == 1) {
-    Part pt{0, C, h->stream, -1};
-    return fn(pt);
-  }
-  DN_CUDA(cudaEventRecord(h->dense_fork, h->stream));
-  int rc = 0;
-  for (int k = 0; k < parts; ++k) {
-    const int c0 = (int)((long long)C * k / parts) & ~255, c1 = (k + 1 == parts) ? C : ((int)((long long)C * (k + 1) / parts) & ~255);
-    Part pt{c0, c1 - c0, h->dense_stream[k], k};
-    DN_CUDA(cudaStreamWaitEvent(pt.st, h->dense_fork, 0));
-    if (rc == 0) rc = fn(pt);
-    DN_CUDA(cudaEventRecord(h->dense_join[k], pt.st));
-    DN_CUDA(cudaStreamWaitEvent(h->stream, h->dense_join[k], 0));
-  }
-  return rc;
 }
 
 // What the product's epilogue emits besides Y: nothing, or the operand planes of Y as variable `var` (PL_P / PL_Q)
@@ -445,31 +391,28 @@ struct PlanesOut {
   int phase;
 };
 
-// Y[c,:] = alpha_c * (X . A^T)[c,:] + beta * Cin[c,:] for the slice, alpha_c = alpha * alpha_dev[c] (or alpha), A one of the
-// handle's constant matrices (float32-accurate, bjx_gemm.cu).  X (when not null) is split exactly into the planes of
-// variable `xvar` first; X == null: the planes of `xvar` are current.  X, Y, Cin, alpha_dev are FULL [C,D] / [C]
-// arrays; the slice's rows are addressed here.
+// Y[c,:] = alpha_c * (X . A^T)[c,:] + beta * Cin[c,:] for the first n rows, alpha_c = alpha * alpha_dev[c] (or alpha), A one
+// of the handle's constant matrices (float32-accurate, bjx_gemm.cu).  X (when not null) is split exactly into the planes of
+// variable `xvar` first; X == null: the planes of `xvar` are current.
 // double_kick: Y = alpha_c acc + (alpha_c acc + Cin) instead (the two half kicks between consecutive leapfrog steps).
-static int gemm(bjx_handle_t h, DenseWs& w, const Part& pt, const float* X, int xvar, int mat, float* Y, const float* Cin,
+static int gemm(bjx_handle_t h, DenseWs& w, int n, const float* X, int xvar, int mat, float* Y, const float* Cin,
                 float alpha, const float* alpha_dev, float beta, bool double_kick = false, PlanesOut po = PlanesOut{-1, 0}) {
   const int D = h->cfg.dim, C = h->cfg.n_chains;
-  const size_t ro = (size_t)pt.c0 * D;
   const int KP = plane_stride(D);
-  uint16_t* xs = w.xs[xvar] + (size_t)pt.c0 * 2 * KP;
   if (X) {
-    k_rows_split2<<<grow(pt.n), kRowWarps * 32, 0, pt.st>>>(pt.n, D, X + ro, xs, w.unscale[xvar] + pt.c0, nullptr, nullptr);
-    DN_LAUNCH("k_rows_split2");
+    k_rows_split2<<<grow(n), kRowWarps * 32, 0, h->stream>>>(n, D, X, w.xs[xvar], w.unscale[xvar], nullptr, nullptr);
+    BJX_CHECK_LAUNCH("k_rows_split2");
   }
   GemmCall g;
-  g.x_planes = xs;
+  g.x_planes = w.xs[xvar];
   g.a_planes = h->dense_mat_s[mat];
-  g.Y = Y + ro;
-  g.Cin = Cin ? Cin + ro : nullptr;
+  g.Y = Y;
+  g.Cin = Cin;
   g.planes_out = nullptr;
-  g.M = pt.n; g.N = D; g.K = D; g.KP = KP; g.KP_out = KP;
+  g.M = n; g.N = D; g.K = D; g.KP = KP; g.KP_out = KP;
   g.epi.alpha = alpha;
-  g.epi.alpha_dev = alpha_dev ? alpha_dev + pt.c0 : nullptr;
-  g.epi.x_unscale = w.unscale[xvar] + pt.c0;
+  g.epi.alpha_dev = alpha_dev;
+  g.epi.x_unscale = w.unscale[xvar];
   g.epi.mat_unscale = w.mat_unscale + mat;
   g.epi.beta = beta;
   g.epi.has_cin = Cin ? 1 : 0;
@@ -478,107 +421,93 @@ static int gemm(bjx_handle_t h, DenseWs& w, const Part& pt, const float* X, int 
   g.epi.out_unscale = nullptr; g.epi.stale_max = nullptr; g.epi.next_max = nullptr; g.epi.zero_max = nullptr;
   if (po.var >= 0) {
     float* ring = w.rmax[po.var];
-    g.planes_out = w.xs[po.var] + (size_t)pt.c0 * 2 * KP;
+    g.planes_out = w.xs[po.var];
     g.epi.planes = 1;
-    g.epi.out_unscale = w.unscale[po.var] + pt.c0;
-    g.epi.stale_max = ring + (size_t)(po.phase % 3) * C + pt.c0;
-    g.epi.next_max = ring + (size_t)((po.phase + 1) % 3) * C + pt.c0;
-    g.epi.zero_max = ring + (size_t)((po.phase + 2) % 3) * C + pt.c0;
+    g.epi.out_unscale = w.unscale[po.var];
+    g.epi.stale_max = ring + (size_t)(po.phase % 3) * C;
+    g.epi.next_max = ring + (size_t)((po.phase + 1) % 3) * C;
+    g.epi.zero_max = ring + (size_t)((po.phase + 2) % 3) * C;
   }
-  const int rc = gemm_f16x3(g, pt.st);
+  const int rc = gemm_f16x3(g, h->stream);
   if (rc) return bjx_fail(h, BJX_E_UNSUPPORTED, "tensor-core product failed (stage " + std::to_string(rc) + ")");
   if (po.var >= 0) {  // rows whose lift left the exact window are re-split from Y (none in a stable trajectory)
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((pt.n + 255) / 256);
+    cfg.gridDim = dim3((n + 255) / 256);
     cfg.blockDim = dim3(256);
-    cfg.stream = pt.st;
+    cfg.stream = h->stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    DN_CUDA(cudaLaunchKernelEx(&cfg, k_planes_fixup, pt.n, D, (const float*)(Y + ro), g.planes_out, g.epi.stale_max,
-                               (const float*)g.epi.next_max, g.epi.out_unscale));
+    BJX_CUDA(cudaLaunchKernelEx(&cfg, k_planes_fixup, n, D, (const float*)Y, g.planes_out, g.epi.stale_max,
+                                (const float*)g.epi.next_max, g.epi.out_unscale));
   }
   return 0;
 }
 
 // v = M^-1 p   (p_presplit: the planes of p are current)
-static int dense_velocity(bjx_handle_t h, DenseWs& w, const Part& pt, const float* p, float* v, bool p_presplit = false) {
+static int dense_velocity(bjx_handle_t h, DenseWs& w, int n, const float* p, float* v, bool p_presplit = false) {
   const int D = h->cfg.dim;
-  if (h->metric_kind == BJX_METRIC_DENSE) return gemm(h, w, pt, p_presplit ? nullptr : p, PL_P, MAT_IMM, v, nullptr, 1.f, nullptr, 0.f);
+  if (h->metric_kind == BJX_METRIC_DENSE) return gemm(h, w, n, p_presplit ? nullptr : p, PL_P, MAT_IMM, v, nullptr, 1.f, nullptr, 0.f);
   const bool per_chain = (h->metric_kind == BJX_METRIC_DIAG_PER_CHAIN);
-  const size_t ro = (size_t)pt.c0 * D;
-  k_rows_scale<<<g4((long long)pt.n * D / 4), 256, 0, pt.st>>>(pt.n, D, h->imm + (per_chain ? ro : 0), per_chain ? D : 0,
-                                                              p + ro, v + ro);
-  DN_LAUNCH("k_rows_scale");
+  k_rows_scale<<<g4((long long)n * D / 4), 256, 0, h->stream>>>(n, D, h->imm, per_chain ? D : 0, p, v);
+  BJX_CHECK_LAUNCH("k_rows_scale");
   return 0;
 }
 
 // g, logp = value_and_grad(q); optionally p += eh * g (once or twice).  q_presplit: the planes of q are current.
 // split_p: also leave the exact planes of the kicked p (for the next M^-1 p product).
-static int dense_grad(bjx_handle_t h, DenseWs& w, const Part& pt, const float* q, float* p, float eps, const float* eps_dev,
+static int dense_grad(bjx_handle_t h, DenseWs& w, int n, const float* q, float* p, float eps, const float* eps_dev,
                       float* g, float* logp, int kicks = 1, bool split_p = false, bool q_presplit = false) {
   const int D = h->cfg.dim;
   const bjx_target_desc& t = h->cfg.target;
-  const size_t ro = (size_t)pt.c0 * D;
-  const float* ed = eps_dev ? eps_dev + pt.c0 : nullptr;
-  float* pp = p ? p + ro : nullptr;
-  uint16_t* ps = (split_p && pp) ? w.xs[PL_P] + (size_t)pt.c0 * 2 * plane_stride(D) : nullptr;
+  uint16_t* ps = (split_p && p) ? w.xs[PL_P] : nullptr;
   if (t.kind == BJX_TARGET_DENSE_GAUSSIAN) {
     // g = -(q P): the sign rides on the product's epilogue
-    int rc = gemm(h, w, pt, q_presplit ? nullptr : q, PL_Q, MAT_PREC, g, nullptr, -1.f, nullptr, 0.f);
+    int rc = gemm(h, w, n, q_presplit ? nullptr : q, PL_Q, MAT_PREC, g, nullptr, -1.f, nullptr, 0.f);
     if (rc) return rc;
-    k_rows_grad_kick<2><<<grow(pt.n), kRowWarps * 32, 0, pt.st>>>(pt.n, D, q + ro, g + ro, nullptr, nullptr, t.logp_offset,
-                                                                pp, eps, ed, g + ro, logp + pt.c0, kicks, ps,
-                                                                w.unscale[PL_P] + pt.c0);
+    k_rows_grad_kick<2><<<grow(n), kRowWarps * 32, 0, h->stream>>>(n, D, q, g, nullptr, nullptr, t.logp_offset, p, eps, eps_dev,
+                                                                 g, logp, kicks, ps, w.unscale[PL_P]);
   } else if (t.kind == BJX_TARGET_DIAG_GAUSSIAN) {
-    k_rows_grad_kick<0><<<grow(pt.n), kRowWarps * 32, 0, pt.st>>>(pt.n, D, q + ro, nullptr, t.inv_var, t.mean, t.logp_offset,
-                                                                pp, eps, ed, g + ro, logp + pt.c0, kicks, ps,
-                                                                w.unscale[PL_P] + pt.c0);
+    k_rows_grad_kick<0><<<grow(n), kRowWarps * 32, 0, h->stream>>>(n, D, q, nullptr, t.inv_var, t.mean, t.logp_offset, p, eps,
+                                                                 eps_dev, g, logp, kicks, ps, w.unscale[PL_P]);
   } else {
     return bjx_fail(h, BJX_E_UNSUPPORTED, "large-D dense path supports DENSE_GAUSSIAN and DIAG_GAUSSIAN targets");
   }
-  DN_LAUNCH("k_rows_grad_kick");
+  BJX_CHECK_LAUNCH("k_rows_grad_kick");
   return 0;
 }
 
-static int dense_momentum(bjx_handle_t h, DenseWs& w, const Part& pt, const uint32_t* keys, float* p_out, bool split_first) {
+static int dense_momentum(bjx_handle_t h, DenseWs& w, int n, const uint32_t* keys, float* p_out, bool split_first) {
   const int D = h->cfg.dim;
-  const size_t ro = (size_t)pt.c0 * D;
   const bool dense_m = (h->metric_kind == BJX_METRIC_DENSE);
   float* z = dense_m ? w.v : p_out;
-  const uint32_t* kp = h->key_shared ? keys : keys + 2 * (size_t)pt.c0;
-  k_dense_normal<<<g4((long long)pt.n * D / 4), 256, 0, pt.st>>>(pt.n, D, kp, z + ro, split_first, h->key_shared,
-                                                                h->chain_offset + (uint32_t)pt.c0);
-  DN_LAUNCH("k_dense_normal");
-  if (dense_m) return gemm(h, w, pt, z, PL_P, MAT_MSQRT, p_out, nullptr, 1.f, nullptr, 0.f);  // p = L^-T z
+  k_dense_normal<<<g4((long long)n * D / 4), 256, 0, h->stream>>>(n, D, keys, z, split_first, h->key_shared, h->chain_offset);
+  BJX_CHECK_LAUNCH("k_dense_normal");
+  if (dense_m) return gemm(h, w, n, z, PL_P, MAT_MSQRT, p_out, nullptr, 1.f, nullptr, 0.f);  // p = L^-T z
   const bool per_chain = (h->metric_kind == BJX_METRIC_DIAG_PER_CHAIN);
-  k_rows_scale<<<g4((long long)pt.n * D / 4), 256, 0, pt.st>>>(pt.n, D, h->msqrt + (per_chain ? ro : 0), per_chain ? D : 0,
-                                                              z + ro, p_out + ro);
-  DN_LAUNCH("k_rows_scale");
+  k_rows_scale<<<g4((long long)n * D / 4), 256, 0, h->stream>>>(n, D, h->msqrt, per_chain ? D : 0, z, p_out);
+  BJX_CHECK_LAUNCH("k_rows_scale");
   return 0;
 }
 
-static int dense_energy(bjx_handle_t h, DenseWs& w, const Part& pt, const float* p, const float* logp, float* e_out,
+static int dense_energy(bjx_handle_t h, DenseWs& w, int n, const float* p, const float* logp, float* e_out,
                         bool p_presplit = false) {
   const int D = h->cfg.dim;
-  int rc = dense_velocity(h, w, pt, p, w.v, p_presplit);
+  int rc = dense_velocity(h, w, n, p, w.v, p_presplit);
   if (rc) return rc;
-  const size_t ro = (size_t)pt.c0 * D;
-  k_rows_energy<<<grow(pt.n), kRowWarps * 32, 0, pt.st>>>(pt.n, D, w.v + ro, p + ro, logp + pt.c0, e_out + pt.c0, 1.f);
-  DN_LAUNCH("k_rows_energy");
+  k_rows_energy<<<grow(n), kRowWarps * 32, 0, h->stream>>>(n, D, w.v, p, logp, e_out, 1.f);
+  BJX_CHECK_LAUNCH("k_rows_energy");
   return 0;
 }
 
-// n velocity-Verlet steps in place (integrators.py:104-150).  p_planes_after: leave the exact planes of the final p
-// (the caller's next product is M^-1 p for the kinetic energy).
-static int dense_leapfrog_core(bjx_handle_t h, DenseWs& w, const Part& pt, float* q, float* p, float* logp, float* g,
-                               float eps, const float* eps_dev, int n_steps, bool p_planes_after = false) {
+// n_steps velocity-Verlet steps in place on all chains (integrators.py:104-150).  p_planes_after: leave the exact planes
+// of the final p (the caller's next product is M^-1 p for the kinetic energy).
+static int dense_leapfrog_core(bjx_handle_t h, DenseWs& w, float* q, float* p, float* logp, float* g, float eps,
+                               const float* eps_dev, int n_steps, bool p_planes_after = false) {
   const int D = h->cfg.dim, C = h->cfg.n_chains;
-  const long long n4 = (long long)pt.n * D / 4;
-  const size_t ro = (size_t)pt.c0 * D;
-  const float* ed = eps_dev ? eps_dev + pt.c0 : nullptr;
+  const long long n4 = (long long)C * D / 4;
   const bool dense_m = (h->metric_kind == BJX_METRIC_DENSE);
   const bool dense_t = (h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN);
   if (n_steps <= 0) return 0;
@@ -587,50 +516,48 @@ static int dense_leapfrog_core(bjx_handle_t h, DenseWs& w, const Part& pt, float
     //   q <- q + eps_c (p M^-1)            reads planes(p), Cin = q, emits planes(q)
     //   p <- p - (eps_c/2)(q P) twice       reads planes(q), Cin = p, emits planes(p)      (between two steps)
     // Only the opening half kick and the closing gradient / logp / half kick are row kernels.
-    const int KP = plane_stride(D);
-    float *pr = w.rmax[PL_P] + pt.c0, *qr = w.rmax[PL_Q] + pt.c0;
-    k_rows_open<<<grow(pt.n), kRowWarps * 32, 0, pt.st>>>(pt.n, D, p + ro, g + ro, q + ro, eps, ed,
-                                                         w.xs[PL_P] + (size_t)pt.c0 * 2 * KP, w.unscale[PL_P] + pt.c0, pr, pr + C,
-                                                         qr, qr + C);
-    DN_LAUNCH("k_rows_open");
+    float *pr = w.rmax[PL_P], *qr = w.rmax[PL_Q];
+    k_rows_open<<<grow(C), kRowWarps * 32, 0, h->stream>>>(C, D, p, g, q, eps, eps_dev, w.xs[PL_P], w.unscale[PL_P], pr, pr + C,
+                                                          qr, qr + C);
+    BJX_CHECK_LAUNCH("k_rows_open");
     int pphase = 0, qphase = 0;
     for (int s = 0; s < n_steps; ++s) {
-      int rc = gemm(h, w, pt, nullptr, PL_P, MAT_IMM, q, q, eps_dev ? 1.0f : eps * 1.0f, eps_dev, 1.f, false, PlanesOut{PL_Q, qphase++});
+      int rc = gemm(h, w, C, nullptr, PL_P, MAT_IMM, q, q, eps_dev ? 1.0f : eps * 1.0f, eps_dev, 1.f, false, PlanesOut{PL_Q, qphase++});
       if (rc) return rc;
       if (s + 1 < n_steps) {
         // Between two steps neither g nor logp is observable, only p += (eps_c/2) g twice (this step's second half kick
         // and the next step's first, integrators.py:134-141,235-239) with g = -(q P): both FMAs ride on the epilogue of
         // the gradient product, per-row factor -(eps_c * 0.5) (bit-identical to kicking with the stored gradient, since
         // the row lifts are powers of two).
-        rc = gemm(h, w, pt, nullptr, PL_Q, MAT_PREC, p, p, eps_dev ? -0.5f : -(eps * 0.5f), eps_dev, 1.f, true, PlanesOut{PL_P, pphase++});
+        rc = gemm(h, w, C, nullptr, PL_Q, MAT_PREC, p, p, eps_dev ? -0.5f : -(eps * 0.5f), eps_dev, 1.f, true, PlanesOut{PL_P, pphase++});
         if (rc) return rc;
       } else {
-        rc = dense_grad(h, w, pt, q, p, eps, eps_dev, g, logp, 1, p_planes_after, true);
+        rc = dense_grad(h, w, C, q, p, eps, eps_dev, g, logp, 1, p_planes_after, true);
         if (rc) return rc;
       }
     }
     return 0;
   }
-  k_rows_axpy<<<g4(n4), 256, 0, pt.st>>>(pt.n, D, p + ro, g + ro, eps, ed, 0.5f);  // first half kick p += (eps/2) g
-  DN_LAUNCH("k_rows_axpy");
+  k_rows_axpy<<<g4(n4), 256, 0, h->stream>>>(C, D, p, g, eps, eps_dev, 0.5f);  // first half kick p += (eps/2) g
+  BJX_CHECK_LAUNCH("k_rows_axpy");
   bool p_presplit = false;
   for (int s = 0; s < n_steps; ++s) {
     int rc;
     if (dense_m) {
       // q = q + (eps_c * 1.0) * (p M^-1): the axpy rides on the product's epilogue
-      rc = gemm(h, w, pt, p_presplit ? nullptr : p, PL_P, MAT_IMM, q, q, eps_dev ? 1.0f : eps * 1.0f, eps_dev, 1.f);
+      rc = gemm(h, w, C, p_presplit ? nullptr : p, PL_P, MAT_IMM, q, q, eps_dev ? 1.0f : eps * 1.0f, eps_dev, 1.f);
       if (rc) return rc;
     } else {
-      rc = dense_velocity(h, w, pt, p, w.v);
+      rc = dense_velocity(h, w, C, p, w.v);
       if (rc) return rc;
-      k_rows_axpy<<<g4(n4), 256, 0, pt.st>>>(pt.n, D, q + ro, w.v + ro, eps, ed, 1.0f);
-      DN_LAUNCH("k_rows_axpy");
+      k_rows_axpy<<<g4(n4), 256, 0, h->stream>>>(C, D, q, w.v, eps, eps_dev, 1.0f);
+      BJX_CHECK_LAUNCH("k_rows_axpy");
     }
     const bool more = (s + 1 < n_steps);
     // g, logp at the new q; p += (eps/2) g; plus the next step's first half kick -- and, with a dense metric, the
     // operand planes of that step's M^-1 p product -- when one follows
     const bool want_planes = dense_m && (more || p_planes_after);
-    rc = dense_grad(h, w, pt, q, p, eps, eps_dev, g, logp, more ? 2 : 1, want_planes);
+    rc = dense_grad(h, w, C, q, p, eps, eps_dev, g, logp, more ? 2 : 1, want_planes);
     if (rc) return rc;
     p_presplit = want_planes;
   }
@@ -640,78 +567,32 @@ static int dense_leapfrog_core(bjx_handle_t h, DenseWs& w, const Part& pt, float
 int bjx_dense_velocity(bjx_handle_t h, const float* p, float* v) {
   DenseWs w;
   int rc = dense_ws(h, w);
-  if (rc) return rc;
-  return for_parts(h, [&](const Part& pt) { return dense_velocity(h, w, pt, p, v); });
+  return rc ? rc : dense_velocity(h, w, h->cfg.n_chains, p, v);
 }
 
 int bjx_dense_init_state(bjx_handle_t h, const float* q, float* logp_out, float* grad_out) {
   DenseWs w;
   int rc = dense_ws(h, w);
-  if (rc) return rc;
-  return for_parts(h, [&](const Part& pt) { return dense_grad(h, w, pt, q, nullptr, 0.f, nullptr, grad_out, logp_out); });
+  return rc ? rc : dense_grad(h, w, h->cfg.n_chains, q, nullptr, 0.f, nullptr, grad_out, logp_out);
 }
 
 int bjx_dense_sample_momentum(bjx_handle_t h, const uint32_t* keys, float* p_out, bool split_first) {
   DenseWs w;
   int rc = dense_ws(h, w);
-  if (rc) return rc;
-  return for_parts(h, [&](const Part& pt) { return dense_momentum(h, w, pt, keys, p_out, split_first); });
+  return rc ? rc : dense_momentum(h, w, h->cfg.n_chains, keys, p_out, split_first);
 }
 
 int bjx_dense_energy(bjx_handle_t h, const float* p, const float* logp, float* e_out) {
   DenseWs w;
   int rc = dense_ws(h, w);
-  if (rc) return rc;
-  return for_parts(h, [&](const Part& pt) { return dense_energy(h, w, pt, p, logp, e_out); });
+  return rc ? rc : dense_energy(h, w, h->cfg.n_chains, p, logp, e_out);
 }
 
 int bjx_dense_leapfrog(bjx_handle_t h, float* q, float* p, float* logp, float* g, float eps, const float* eps_dev,
                        int n_steps) {
   DenseWs w;
   int rc = dense_ws(h, w);
-  if (rc) return rc;
-  return for_parts(h, [&](const Part& pt) { return dense_leapfrog_core(h, w, pt, q, p, logp, g, eps, eps_dev, n_steps); });
-}
-
-static int dense_hmc_part(bjx_handle_t h, DenseWs& w, const Part& pt, const uint32_t* keys, const float* q_in,
-                          const float* logp_in, const float* g_in, float* q_out, float* logp_out, float* g_out, float eps,
-                          const float* eps_dev, int L, const InfoPtrs& info) {
-  const int D = h->cfg.dim;
-  const size_t ro = (size_t)pt.c0 * D;
-  const size_t bytes = (size_t)pt.n * D * sizeof(float);
-  int rc = dense_momentum(h, w, pt, keys, w.p, true);  // hmc.py:299-302
-  if (rc) return rc;
-  if (info.momentum) DN_CUDA(cudaMemcpyAsync(info.momentum + ro, w.p + ro, bytes, cudaMemcpyDeviceToDevice, pt.st));
-  rc = dense_energy(h, w, pt, w.p, logp_in, w.e0);  // hmc.py:159
-  if (rc) return rc;
-  DN_CUDA(cudaMemcpyAsync(w.q + ro, q_in + ro, bytes, cudaMemcpyDeviceToDevice, pt.st));
-  DN_CUDA(cudaMemcpyAsync(w.g + ro, g_in + ro, bytes, cudaMemcpyDeviceToDevice, pt.st));
-  DN_CUDA(cudaMemcpyAsync(w.lw + pt.c0, logp_in + pt.c0, (size_t)pt.n * sizeof(float), cudaMemcpyDeviceToDevice, pt.st));
-  const bool planes_after = (h->metric_kind == BJX_METRIC_DENSE) && L > 0;
-  rc = dense_leapfrog_core(h, w, pt, w.q, w.p, w.lw, w.g, eps, eps_dev, L, planes_after);  // trajectory.py:165
-  if (rc) return rc;
-  // kinetic energy of the (flipped) end momentum: (-p)^T M^-1 (-p) = p^T M^-1 p   (hmc.py:158-160)
-  rc = dense_energy(h, w, pt, w.p, w.lw, w.e1, planes_after);
-  if (rc) return rc;
-  if (info.proposal_position) DN_CUDA(cudaMemcpyAsync(info.proposal_position + ro, w.q + ro, bytes, cudaMemcpyDeviceToDevice, pt.st));
-  if (info.proposal_momentum) {  // flipped momentum (hmc.py:158)
-    DN_CUDA(cudaMemsetAsync(info.proposal_momentum + ro, 0, bytes, pt.st));
-    k_rows_axpy<<<g4((long long)pt.n * D / 4), 256, 0, pt.st>>>(pt.n, D, info.proposal_momentum + ro, w.p + ro, -1.0f, nullptr, 1.0f);
-    DN_LAUNCH("k_rows_axpy");
-  }
-  InfoPtrs ip = info;  // per-chain outputs of this slice
-  if (ip.acceptance_rate) ip.acceptance_rate += pt.c0;
-  if (ip.is_accepted) ip.is_accepted += pt.c0;
-  if (ip.is_divergent) ip.is_divergent += pt.c0;
-  if (ip.energy) ip.energy += pt.c0;
-  if (ip.num_integration_steps) ip.num_integration_steps += pt.c0;
-  const uint32_t* kp = h->key_shared ? keys : keys + 2 * (size_t)pt.c0;
-  k_rows_accept<<<grow(pt.n), kRowWarps * 32, 0, pt.st>>>(pt.n, D, kp, w.e0 + pt.c0, w.e1 + pt.c0, h->cfg.divergence_threshold,
-                                                         w.q + ro, w.g + ro, w.lw + pt.c0, q_in + ro, g_in + ro, logp_in + pt.c0,
-                                                         q_out + ro, g_out + ro, logp_out + pt.c0, L, ip, h->key_shared,
-                                                         h->chain_offset + (uint32_t)pt.c0);
-  DN_LAUNCH("k_rows_accept");
-  return 0;
+  return rc ? rc : dense_leapfrog_core(h, w, q, p, logp, g, eps, eps_dev, n_steps);
 }
 
 int bjx_dense_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, const float* g_in,
@@ -720,9 +601,33 @@ int bjx_dense_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, 
   DenseWs w;
   int rc = dense_ws(h, w);
   if (rc) return rc;
-  return for_parts(h, [&](const Part& pt) {
-    return dense_hmc_part(h, w, pt, keys, q_in, logp_in, g_in, q_out, logp_out, g_out, eps, eps_dev, L, info);
-  });
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  const size_t bytes = (size_t)C * D * sizeof(float);
+  rc = dense_momentum(h, w, C, keys, w.p, true);  // hmc.py:299-302
+  if (rc) return rc;
+  if (info.momentum) BJX_CUDA(cudaMemcpyAsync(info.momentum, w.p, bytes, cudaMemcpyDeviceToDevice, h->stream));
+  rc = dense_energy(h, w, C, w.p, logp_in, w.e0);  // hmc.py:159
+  if (rc) return rc;
+  BJX_CUDA(cudaMemcpyAsync(w.q, q_in, bytes, cudaMemcpyDeviceToDevice, h->stream));
+  BJX_CUDA(cudaMemcpyAsync(w.g, g_in, bytes, cudaMemcpyDeviceToDevice, h->stream));
+  BJX_CUDA(cudaMemcpyAsync(w.lw, logp_in, (size_t)C * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  const bool planes_after = (h->metric_kind == BJX_METRIC_DENSE) && L > 0;
+  rc = dense_leapfrog_core(h, w, w.q, w.p, w.lw, w.g, eps, eps_dev, L, planes_after);  // trajectory.py:165
+  if (rc) return rc;
+  // kinetic energy of the (flipped) end momentum: (-p)^T M^-1 (-p) = p^T M^-1 p   (hmc.py:158-160)
+  rc = dense_energy(h, w, C, w.p, w.lw, w.e1, planes_after);
+  if (rc) return rc;
+  if (info.proposal_position) BJX_CUDA(cudaMemcpyAsync(info.proposal_position, w.q, bytes, cudaMemcpyDeviceToDevice, h->stream));
+  if (info.proposal_momentum) {  // flipped momentum (hmc.py:158)
+    BJX_CUDA(cudaMemsetAsync(info.proposal_momentum, 0, bytes, h->stream));
+    k_rows_axpy<<<g4((long long)C * D / 4), 256, 0, h->stream>>>(C, D, info.proposal_momentum, w.p, -1.0f, nullptr, 1.0f);
+    BJX_CHECK_LAUNCH("k_rows_axpy");
+  }
+  k_rows_accept<<<grow(C), kRowWarps * 32, 0, h->stream>>>(C, D, keys, w.e0, w.e1, h->cfg.divergence_threshold, w.q, w.g, w.lw,
+                                                          q_in, g_in, logp_in, q_out, g_out, logp_out, L, info, h->key_shared,
+                                                          h->chain_offset);
+  BJX_CHECK_LAUNCH("k_rows_accept");
+  return 0;
 }
 
 #include "bjx_dense_nuts.cuh"

@@ -288,12 +288,8 @@ static int dn_ws(bjx_handle_t h, DnWs& dn) {
   const size_t C = h->cfg.n_chains, D = h->cfg.dim, depth = h->cfg.max_tree_depth;
   const size_t row = ((C * D * sizeof(float)) + 255) & ~(size_t)255, vec = ((C * sizeof(float)) + 255) & ~(size_t)255;
   const size_t need = (7 + depth) * row + 12 * vec + 256;
-  if (h->dn_bytes < need) {
-    if (h->dn_block) DN_CUDA(cudaFree(h->dn_block));
-    h->dn_block = nullptr;
-    DN_CUDA(cudaMalloc(&h->dn_block, need));
-    h->dn_bytes = need;
-  }
+  int rc = bjx_grow(h, h->dn_block, h->dn_bytes, need, 1);
+  if (rc) return rc;
   char* b = (char*)h->dn_block;
   auto take = [&](size_t bytes) { char* r = b; b += bytes; return r; };
   dn.cq = (float*)take(row); dn.cp = (float*)take(row); dn.cg = (float*)take(row); dn.cv = (float*)take(row);
@@ -316,7 +312,7 @@ int bjx_dense_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* q_in,
                         float* q_out, float* logp_out, float* g_out, float step_size, const float* step_size_dev,
                         int max_num_doublings, InfoPtrs info, const float* momentum_override,
                         const uint32_t* key_integrator_override) {
-  DN_CUDA(cudaSetDevice(h->cfg.device));
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   int rc = bjx_ensure_nuts_ws(h);
   if (rc) return rc;
@@ -329,60 +325,58 @@ int bjx_dense_nuts_step(bjx_handle_t h, const uint32_t* keys, const float* q_in,
   NutsWs& ws = h->ws;
   cudaStream_t st = h->stream;
   const bool dense_m = (h->metric_kind == BJX_METRIC_DENSE);
-  Part all{0, C, st, -1};
-  DN_CUDA(cudaMemsetAsync(ws.counters, 0, 64 * sizeof(int), st));
+  BJX_CUDA(cudaMemsetAsync(ws.counters, 0, 64 * sizeof(int), st));
   // momentum draw (nuts.py:136) and its velocity
   if (momentum_override) {
-    DN_CUDA(cudaMemcpyAsync(ws.left_p, momentum_override, (size_t)C * D * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    BJX_CUDA(cudaMemcpyAsync(ws.left_p, momentum_override, (size_t)C * D * sizeof(float), cudaMemcpyDeviceToDevice, st));
   } else {
-    rc = dense_momentum(h, w, all, keys, ws.left_p, true);
+    rc = dense_momentum(h, w, C, keys, ws.left_p, true);
     if (rc) return rc;
   }
-  rc = dense_velocity(h, w, all, ws.left_p, dn.left_v);
+  rc = dense_velocity(h, w, C, ws.left_p, dn.left_v);
   if (rc) return rc;
   k_dn_init<<<grow(C), kRowWarps * 32, 0, st>>>(C, D, ws, dn, keys, h->key_shared, h->chain_offset, key_integrator_override, q_in,
                                                 logp_in, g_in, q_out, logp_out, g_out, info.momentum);
-  DN_LAUNCH("k_dn_init");
+  BJX_CHECK_LAUNCH("k_dn_init");
 
   int n = C;
   const int* list = nullptr;
   int64_t launches = 0;
   for (int d = 0; d < max_num_doublings && n > 0; ++d) {
-    Part pt{0, n, st, -1};
     uint16_t* planes = dense_m ? w.xs[PL_P] : nullptr;
     k_dn_begin<<<grow(n), kRowWarps * 32, 0, st>>>(n, D, d, ws, dn, list, step_size, step_size_dev, planes, w.unscale[PL_P]);
-    DN_LAUNCH("k_dn_begin");
+    BJX_CHECK_LAUNCH("k_dn_begin");
     const int leaves = 1 << d;
     for (int i = 0; i < leaves; ++i) {
       // half-step velocity, position update (integrators.py:199-203,242)
-      rc = dense_velocity(h, w, pt, dn.cp, w.v, dense_m);
+      rc = dense_velocity(h, w, n, dn.cp, w.v, dense_m);
       if (rc) return rc;
       k_rows_axpy<<<g4((long long)n * D / 4), 256, 0, st>>>(n, D, dn.cq, w.v, 0.f, dn.ceps, 1.0f);
-      DN_LAUNCH("k_rows_axpy");
+      BJX_CHECK_LAUNCH("k_rows_axpy");
       // gradient, log density, second half kick (and the planes of the full-step momentum)
-      rc = dense_grad(h, w, pt, dn.cq, dn.cp, 0.f, dn.ceps, dn.cg, dn.clogp, 1, dense_m, false);
+      rc = dense_grad(h, w, n, dn.cq, dn.cp, 0.f, dn.ceps, dn.cg, dn.clogp, 1, dense_m, false);
       if (rc) return rc;
       // full-step velocity: kinetic energy and the U-turn tests of this leaf
-      rc = dense_velocity(h, w, pt, dn.cp, dn.cv, dense_m);
+      rc = dense_velocity(h, w, n, dn.cp, dn.cv, dense_m);
       if (rc) return rc;
       k_dn_leaf<<<grow(n), kRowWarps * 32, 0, st>>>(n, D, i, leaves - 1, C, ws, dn, list, h->cfg.divergence_threshold, planes,
                                                     w.unscale[PL_P]);
-      DN_LAUNCH("k_dn_leaf");
+      BJX_CHECK_LAUNCH("k_dn_leaf");
       ++launches;
     }
     int* list_out = (d & 1) ? ws.list_b : ws.list_a;
     k_dn_end<<<grow(n), kRowWarps * 32, 0, st>>>(n, D, d, max_num_doublings, ws, dn, list, list_out, ws.counters + 1 + d, q_out,
                                                  logp_out, g_out);
-    DN_LAUNCH("k_dn_end");
+    BJX_CHECK_LAUNCH("k_dn_end");
     if (d + 1 < max_num_doublings) {  // the one host read per doubling: how many chains go on
-      DN_CUDA(cudaMemcpyAsync(h->h_flag, ws.counters + 1 + d, sizeof(int), cudaMemcpyDeviceToHost, st));
-      DN_CUDA(cudaStreamSynchronize(st));
+      BJX_CUDA(cudaMemcpyAsync(h->h_flag, ws.counters + 1 + d, sizeof(int), cudaMemcpyDeviceToHost, st));
+      BJX_CUDA(cudaStreamSynchronize(st));
       n = h->h_flag[0];
       list = list_out;
     }
   }
   k_nuts_finish<<<(C + 255) / 256, 256, 0, st>>>(C, ws, info);
-  DN_LAUNCH("k_nuts_finish");
+  BJX_CHECK_LAUNCH("k_nuts_finish");
   h->last_leaf_launches = launches;
   h->last_depth = -1;
   return 0;

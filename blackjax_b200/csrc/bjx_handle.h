@@ -17,49 +17,45 @@ struct bjx_plugin_s {
 };
 
 struct bjx_handle_s {
-  bjx_config cfg;
-  cudaStream_t stream;
-  int sc;              // SizeClass
-  int metric_kind;     // -1 until set
-  bool metric_small_dense;
-  const float* imm;    // caller-owned
-  float* msqrt;        // owned
-  size_t msqrt_elems;
+  bjx_config cfg{};
+  cudaStream_t stream = nullptr;
+  int sc = 0;                    // SizeClass
+  int metric_kind = -1;          // -1 until set
+  bool metric_small_dense = false;
+  const float* imm = nullptr;    // caller-owned
+  float* msqrt = nullptr;        // owned
+  size_t msqrt_elems = 0;
   // NUTS workspace (owned, lazily allocated)
-  bjx::NutsWs ws;
-  void* ws_block;
-  int ws_depth;
-  int* h_flag;         // pinned
-  int64_t last_leaf_launches, last_depth;
+  bjx::NutsWs ws{};
+  void* ws_block = nullptr;
+  int ws_depth = 0;
+  int* h_flag = nullptr;         // pinned
+  int64_t last_leaf_launches = 0, last_depth = 0;
   // large-D dense path (bjx_dense.cu): working rows p, v, q, g [C,D] + GEMM workspace
-  float* dense_block;
-  size_t dense_bytes;
-  void* gemm_ws;
-  size_t gemm_ws_bytes;
-  uint16_t* dense_mat_s[3];      // fp16-split copies of M^-1, L^-T, target precision ([D, 3D] each)
-  const float* dense_mat_src[3]; // the float32 matrices they were built from
-  unsigned dense_mat_ver[3];
-  unsigned dense_version;        // bumped by bjx_set_metric / bjx_set_target (contents may change behind the same pointer)
-  size_t dense_bytes_built;
-  float* lr_block;               // low-rank metric (owned): U [D,k] | sigma [D] | 1/sigma [D] | lambda-1 [k] | 1/sqrt(lambda)-1 [k]
-  int lr_k;
-  void* dn_block;                // NUTS on the dense path (bjx_dense_nuts.cuh): compact rows, checkpoint velocities
-  size_t dn_bytes;
-  float* pool_scratch;           // scratch of bjx_pooled_stats_dense (slice partials of the D x D co-moment)
-  size_t pool_scratch_bytes;
-  cudaStream_t dense_stream[2];  // chain slices of the dense path run on their own streams (bjx_dense.cu)
-  cudaEvent_t dense_fork, dense_join[2], dense_stagger;
-  bool dense_stagger_armed;
-  bool dense_streams_ready;
-  int ncoef;            // integrator coefficient table (integrators.py:321-369); {0.5, 1, 0.5} = velocity Verlet
-  float coef[11];
-  bool general_integrator;
-  int key_shared;          // see bjx_set_key_mode
-  const int32_t* steps_dev;  // see bjx_set_integration_steps
-  const float* ghmc_noise;   // see bjx_set_ghmc_noise
-  uint32_t chain_offset;
-  uint32_t* sample_keys;   // [num_steps, 2] step keys of bjx_hmc_sample
-  size_t sample_keys_cap;
+  float* dense_block = nullptr;
+  size_t dense_bytes = 0;
+  void* gemm_ws = nullptr;
+  size_t gemm_ws_bytes = 0;
+  uint16_t* dense_mat_s[3] = {};       // fp16-split copies of M^-1, L^-T, target precision ([D, 3D] each)
+  const float* dense_mat_src[3] = {};  // the float32 matrices they were built from
+  unsigned dense_mat_ver[3] = {};
+  unsigned dense_version = 1;    // bumped by bjx_set_metric / bjx_set_target (contents may change behind the same pointer)
+  size_t dense_bytes_built = 0;
+  float* lr_block = nullptr;     // low-rank metric (owned): U [D,k] | sigma [D] | 1/sigma [D] | lambda-1 [k] | 1/sqrt(lambda)-1 [k]
+  int lr_k = 0;
+  void* dn_block = nullptr;      // NUTS on the dense path (bjx_dense_nuts.cuh): compact rows, checkpoint velocities
+  size_t dn_bytes = 0;
+  float* pool_scratch = nullptr; // scratch of bjx_pooled_stats_dense (slice partials of the D x D co-moment)
+  size_t pool_scratch_bytes = 0;
+  int ncoef = 3;                 // integrator coefficient table (integrators.py:321-369); {0.5, 1, 0.5} = velocity Verlet
+  float coef[11] = {0.5f, 1.0f, 0.5f};
+  bool general_integrator = false;
+  int key_shared = 0;                  // see bjx_set_key_mode
+  const int32_t* steps_dev = nullptr;  // see bjx_set_integration_steps
+  const float* ghmc_noise = nullptr;   // see bjx_set_ghmc_noise
+  uint32_t chain_offset = 0;
+  uint32_t* sample_keys = nullptr;     // [num_steps, 2] step keys of the run loops (bjx_hmc_sample, ...)
+  size_t sample_keys_cap = 0;
   std::string err;
 };
 
@@ -67,4 +63,30 @@ int bjx_fail(bjx_handle_t h, int code, const std::string& msg);
 int bjx_ensure_nuts_ws(bjx_handle_t h);  // the NUTS workspace of bjx_api.cu (shared with the dense path)
 int bjx_cuda_fail(bjx_handle_t h, cudaError_t e, const char* where);
 
+// Grow-only device buffer: *buf holds at least `need` units (elements or bytes, as *cap counts them) afterwards.
+template <class T>
+int bjx_grow(bjx_handle_t h, T*& buf, size_t& cap, size_t need, size_t unit_bytes) {
+  if (need <= cap) return 0;
+  if (buf) {
+    cudaError_t e = cudaFree(buf);
+    buf = nullptr;
+    cap = 0;
+    if (e != cudaSuccess) return bjx_cuda_fail(h, e, "cudaFree");
+  }
+  cudaError_t e = cudaMalloc((void**)&buf, need * unit_bytes);
+  if (e != cudaSuccess) return bjx_cuda_fail(h, e, "cudaMalloc");
+  cap = need;
+  return 0;
+}
 
+// Error idiom of every entry point: a failing CUDA call or kernel launch returns its cudaError_t, message in h->err.
+#define BJX_CUDA(call)                                            \
+  do {                                                            \
+    cudaError_t e_ = (call);                                      \
+    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, #call);    \
+  } while (0)
+#define BJX_CHECK_LAUNCH(where)                                   \
+  do {                                                            \
+    cudaError_t e_ = cudaGetLastError();                          \
+    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, where);    \
+  } while (0)

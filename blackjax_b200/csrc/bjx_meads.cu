@@ -295,12 +295,6 @@ static long long next_pow2(long long n) {
 
 using namespace bjx;
 
-#define BJX_CUDA(call)                                       \
-  do {                                                       \
-    cudaError_t e_ = (call);                                 \
-    if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, #call); \
-  } while (0)
-
 extern "C" size_t bjx_meads_state_floats(int32_t num_folds, int32_t dim) {
   return (size_t)3 * num_folds + (size_t)3 * num_folds * dim;
 }

@@ -15,12 +15,9 @@
 #if defined(BJX_PLUGIN_BIG) && BJX_PLUGIN_BIG
 // ---- rows beyond a warp (1024 < dim <= 18432): CTA-per-chain kernels around bjx_user::BigModel ----------------------------
 #include "bjx_big.cuh"
-#include "bjx_launch.cuh"   // (LaunchArgs: part of the ABI number)
 #include BJX_USER_SOURCE
 
-extern "C" int bjx_plugin_built_for_abi(void) {
-  return BJX_VERSION * 100000 + (int)sizeof(bjx::LaunchArgs) + 7 * (int)sizeof(bjx::BigLaunchArgs);
-}
+extern "C" int bjx_plugin_built_for_abi(void) { return bjx::plugin_abi(); }
 // 0 = launched; > 0 = the cudaError_t of the launch
 extern "C" int bjx_plugin_launch_big(int kernel_id, const bjx::BigLaunchArgs* a) {
   return bjx::big_launch<BJX_TARGET_USER>(kernel_id, *a);
@@ -31,12 +28,10 @@ extern "C" int bjx_plugin_launch_big(int kernel_id, const bjx::BigLaunchArgs* a)
 #include BJX_USER_SOURCE
 
 #include "../../include/bjx.h"
-#include "bjx_big.cuh"      // (BigLaunchArgs: part of the ABI number)
+#include "bjx_big.cuh"      // (plugin_abi)
 #include "bjx_launch.cuh"
 
-extern "C" int bjx_plugin_built_for_abi(void) {
-  return BJX_VERSION * 100000 + (int)sizeof(bjx::LaunchArgs) + 7 * (int)sizeof(bjx::BigLaunchArgs);
-}
+extern "C" int bjx_plugin_built_for_abi(void) { return bjx::plugin_abi(); }
 
 // 0 = launched; -2 = this (kernel, row size, metric, integrator) variant was not built into the plug-in; > 0 = the
 // cudaError_t of the launch (the plug-in has its own CUDA runtime instance, so it reports its own launch errors).
