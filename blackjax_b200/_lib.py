@@ -8,6 +8,7 @@ LIB_PATH = os.path.join(_HERE, "libbjx.so")
 
 TARGET_DIAG_GAUSSIAN, TARGET_FUNNEL, TARGET_DENSE_GAUSSIAN, TARGET_BANANA, TARGET_HIER_LOGIT, TARGET_USER = 0, 1, 2, 3, 4, 5
 METRIC_DIAG, METRIC_DENSE, METRIC_DIAG_PER_CHAIN, METRIC_LOW_RANK, METRIC_DENSE_PER_CHAIN = 0, 1, 2, 3, 4
+CHEES_WHITEN, CHEES_LENGTH_FLOOR = 1, 2
 
 _f32p = C.c_void_p  # device pointers travel as integers
 
@@ -105,6 +106,15 @@ _SIGNATURES = {
     "bjx_chees_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_void_p,
                                    C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, _f32p, C.c_void_p, _f32p]),
     "bjx_chees_final": (C.c_int, [C.c_void_p, _f32p, C.POINTER(C.c_float)]),
+    "bjx_chees_metric_state_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "bjx_chees_metric_init": (C.c_int, [C.c_void_p, _f32p, C.c_int32, C.c_int32, _f32p]),
+    "bjx_chees_update_metric": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                          _f32p, _f32p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
+                                          C.c_int32, C.c_int32, C.c_int32, _f32p, C.c_void_p, _f32p, _f32p, _f32p, _f32p]),
+    "bjx_chees_final_metric": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _f32p, _f32p, C.c_int32, _f32p,
+                                         C.POINTER(C.c_float)]),
+    "bjx_chees_metric_fold_covariance": (C.c_int, [C.c_void_p, C.c_int32, _f32p, _f32p]),
+    "bjx_chees_metric_covariance": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _f32p, _f32p]),
     "bjx_ghmc_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, _f32p,
                                 C.c_float, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(Info)]),
     "bjx_meads_state_floats": (C.c_size_t, [C.c_int32, C.c_int32]),

@@ -16,6 +16,8 @@
 #include <dlfcn.h>
 #include <nccl.h>
 
+#include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <mutex>
 #include <string>
@@ -402,6 +404,36 @@ __global__ void k_chees_pass1(int C, int D, const float* __restrict__ prop_q, co
   }
 }
 
+// ---- diagonal-metric mode (mass_matrix_estimation="diagonal", chees_adaptation.py:61-237,758-1001) ----------------
+// Its own state ("metric state", MmLayout below).  Header slots:
+enum { MM_WSTEPS = 0, MM_CG, MM_THRESH, MM_ENGAGED, MM_LAMBDA, MM_WHITEN, MM_FLOOR };
+constexpr int kMmHdr = 16;
+
+// The diagonal Welford accumulator of the reference (mass_matrix.py:364-444, one row at a time) is kept as (n, mean, m2):
+// each in-window step the k_block_stats blocks of the new positions are merged in global block order and the pooled
+// block is merged into the accumulator (Chan-Golub-LeVeque; equal to the sequential fold in exact arithmetic).
+// n = in-window steps * global chain count, formed in double (exact far beyond 2^24 samples).
+__device__ __forceinline__ void mm_fold_diag(int D, int d, int nblk, int nbl, size_t R, size_t off, const float* __restrict__ blocks,
+                                             float* __restrict__ ms) {
+  const size_t S = 2 + 2 * (size_t)D;
+  auto blk = [&](int b) { return blocks + (size_t)(b / nbl) * R + off + (size_t)(b % nbl) * S; };
+  float nn = blk(0)[1], mean = blk(0)[2 + d], m2 = blk(0)[2 + D + d];
+  for (int b = 1; b < nblk; ++b) {
+    const float* g = blk(b);
+    float fm, fc, nab;
+    cgl_factors(nn, g[1], fm, fc, nab);
+    const float delta = g[2 + d] - mean;
+    mean = mean + delta * fm;
+    m2 = m2 + g[2 + D + d] + delta * delta * fc;
+    nn = nab;
+  }
+  const double na = (double)ms[MM_WSTEPS] * (double)ms[MM_CG], nb = (double)nn, ab = na + nb;
+  const float fm = (float)(nb / ab), fc = (float)(na * nb / ab);
+  const float delta = mean - ms[kMmHdr + d];
+  ms[kMmHdr + d] = ms[kMmHdr + d] + delta * fm;
+  ms[kMmHdr + D + d] = ms[kMmHdr + D + d] + m2 + delta * delta * fc;
+}
+
 // merge the pass-1 blocks in global order: proposal mean (weighted), initial mean (nanmean), harmonic-mean sums
 __global__ void k_chees_means(int D, int nblk, const float* __restrict__ blocks, float* __restrict__ st) {
   const size_t S = 3 + 3 * (size_t)D;
@@ -426,22 +458,66 @@ __global__ void k_chees_means(int D, int nblk, const float* __restrict__ blocks,
     st[CH_HM_N] = n;
   }
 }
+// k_chees_means for the diagonal-metric mode: the same sums in the same order over a rank-major payload of R floats per
+// rank, [nbl pass-1 blocks | nbl k_block_stats blocks of the new positions]; with in_window the latter are folded into the
+// diagonal accumulator of `ms`
+__global__ void k_chees_means_metric(int D, int nblk, const float* __restrict__ blocks, float* __restrict__ st, int nbl, size_t R,
+                                     float* __restrict__ ms, int in_window) {
+  const size_t S = 3 + 3 * (size_t)D;
+  auto blk = [&](int b) { return blocks + (size_t)(b / nbl) * R + (size_t)(b % nbl) * S; };
+  float* pm = st + kChHdr;
+  float* qm = pm + D;
+  float sw = 0.f;
+  for (int b = 0; b < nblk; ++b) sw += blk(b)[2];
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    float a = 0.f, q = 0.f, n = 0.f;
+    for (int b = 0; b < nblk; ++b) {
+      a += blk(b)[3 + d];
+      q += blk(b)[3 + D + d];
+      n += blk(b)[3 + 2 * D + d];
+    }
+    pm[d] = a / (sw + 1e-20f);
+    qm[d] = q / n;
+    if (in_window) mm_fold_diag(D, d, nblk, nbl, R, (size_t)nbl * S, blocks, ms);
+  }
+  if (threadIdx.x == 0) {
+    float h = 0.f, n = 0.f;
+    for (int b = 0; b < nblk; ++b) { h += blk(b)[0]; n += blk(b)[1]; }
+    st[CH_HM_SUM] = h;
+    st[CH_HM_N] = n;
+  }
+  __syncthreads();  // every thread has read the sample count
+  if (in_window && threadIdx.x == 0) ms[MM_WSTEPS] += 1.f;
+}
 
-// per chain (one warp): (|x' - E x'|^2 - |x - E x|^2) <x' - E x', p'>, then its acceptance-weighted terms
+// per chain (one warp): (|x' - E x'|^2 - |x - E x|^2) <x' - E x', p'>, then its acceptance-weighted terms.
+// kWhiten (chees_adaptation.py:449-458): x' - E x' and x - E x scaled by 1/sqrt(imm), the momentum by imm then 1/sqrt(imm);
+// with imm = ones every scaling is exact, so the result is bit-identical to the raw expression.
+template <bool kWhiten = false>
 __global__ void k_chees_dots(int C, int D, const float* __restrict__ prop_q, const float* __restrict__ prop_p,
                              const float* __restrict__ init_q, const float* __restrict__ acc, const uint8_t* __restrict__ is_div,
-                             const float* __restrict__ st, float* __restrict__ num, float* __restrict__ den) {
+                             const float* __restrict__ st, float* __restrict__ num, float* __restrict__ den,
+                             const float* __restrict__ imm = nullptr) {
   const int lane = threadIdx.x & 31, c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (c >= C) return;
   const float* pm = st + kChHdr;
   const float* qm = pm + D;
   float a = 0.f, b = 0.f, d = 0.f;
   for (int i = lane; i < D; i += 32) {
-    const float pc = prop_q[(size_t)c * D + i] - pm[i];
-    const float ic = init_q[(size_t)c * D + i] - qm[i];
-    a = fmaf(pc, pc, a);
-    b = fmaf(ic, ic, b);
-    d = fmaf(pc, prop_p[(size_t)c * D + i], d);
+    if constexpr (kWhiten) {
+      const float s = 1.0f / sqrtf(imm[i]);
+      const float pc = (prop_q[(size_t)c * D + i] - pm[i]) * s;
+      const float ic = (init_q[(size_t)c * D + i] - qm[i]) * s;
+      a = fmaf(pc, pc, a);
+      b = fmaf(ic, ic, b);
+      d = fmaf(pc, (prop_p[(size_t)c * D + i] * imm[i]) * s, d);
+    } else {
+      const float pc = prop_q[(size_t)c * D + i] - pm[i];
+      const float ic = init_q[(size_t)c * D + i] - qm[i];
+      a = fmaf(pc, pc, a);
+      b = fmaf(ic, ic, b);
+      d = fmaf(pc, prop_p[(size_t)c * D + i], d);
+    }
   }
   for (int off = 16; off > 0; off >>= 1) {
     a += __shfl_xor_sync(0xffffffffu, a, off);
@@ -474,9 +550,14 @@ __global__ void k_chees_pass2(int C, const float* __restrict__ num, const float*
   }
 }
 
-// the scalar update (chees_adaptation.py:341-360,470-511) and the next transition's step count
+// the scalar update (chees_adaptation.py:341-360,470-511) and the next transition's step count.
+// kMetric: the next transition consumes min(max(T, floor), max_leapfrog * eps) with floor = (pi/2) sqrt(lambda_max) once the
+// diagonal estimate is engaged (_apply_length_floor, :192-236); T itself, the optimiser's state, is never floored.
+template <bool kMetric = false>
 __global__ void k_chees_finish(int nblk, const float* __restrict__ blocks2, float* __restrict__ st, float lr, float b1, float b2,
-                               float target, float decay, float max_leapfrog, float* __restrict__ hist) {
+                               float target, float decay, float max_leapfrog, float* __restrict__ hist,
+                               const float* __restrict__ ms = nullptr, float* __restrict__ lam_hist = nullptr,
+                               float* __restrict__ eng_hist = nullptr) {
   if (threadIdx.x != 0) return;
   const int max_bits = (int)st[CH_MAX_BITS];
   const float jam = st[CH_JITTER_AMOUNT];
@@ -529,9 +610,22 @@ __global__ void k_chees_finish(int nblk, const float* __restrict__ blocks2, floa
   st[CH_GRAD] = grad;
   // next transition: ceil(jitter(i + 1) * T / eps) leapfrog steps (integration_steps_fn :775-779)
   const float jn = halton_f(rga + 1, max_bits) * jam + (1.f - jam);
-  st[CH_L] = ceilf(jn * (newT / eps));
+  if constexpr (kMetric) {
+    float consumed = newT;
+    if (ms[MM_FLOOR] != 0.f) {
+      const float floor_v = ms[MM_ENGAGED] != 0.f ? 1.57079637f * sqrtf(ms[MM_LAMBDA]) : 0.f;
+      consumed = fminf(fmaxf(newT, floor_v), max_leapfrog * eps);
+    }
+    st[CH_L] = ceilf(jn * (consumed / eps));
+  } else {
+    st[CH_L] = ceilf(jn * (newT / eps));
+  }
   const int t = (int)st[CH_T_IDX];
   if (hist) { hist[4 * t] = eps; hist[4 * t + 1] = newT; hist[4 * t + 2] = st[CH_L]; hist[4 * t + 3] = grad; }
+  if constexpr (kMetric) {
+    if (lam_hist) lam_hist[t] = ms[MM_LAMBDA];
+    if (eng_hist) eng_hist[t] = ms[MM_ENGAGED];
+  }
   st[CH_T_IDX] = (float)(t + 1);
 }
 __global__ void k_chees_init(float* st, float eps0, int max_bits, float jitter_amount) {
@@ -546,6 +640,205 @@ __global__ void k_chees_init(float* st, float eps0, int max_bits, float jitter_a
 __global__ void k_fill_steps(int n, const float* __restrict__ src, int32_t* __restrict__ dst) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = (int32_t)src[0];
+}
+
+// ---- windowed covariance accumulator of the length floor (cgl_update_batch, metric_buffers.py:396-447) -------------
+// Every statistic block b of BJX_STAT_BLOCK_CHAINS chains keeps its own (count, mean[D], m2[D, D]) over the window; per
+// in-window step m2_b += X~_b^T X~_b + f delta delta^T with X~_b the block's rows centred on this step's block mean,
+// delta = step mean - accumulated mean, f = n_a n_b / (n_a + n_b).  Only the lower triangle of m2_b is kept.
+//
+// k_cov_syrk: hand-written float32 SIMT SYRK.  grid (lower-triangular 64x64 output tiles, blocks), 256 threads, each
+// thread a 4x4 register tile; the chain axis is staged through shared memory 16 rows at a time, centred (and zero-padded
+// past the block's last chain or the last column) while it is staged, so every C and D <= 1024 takes the same code.  A
+// 16-row chunk is summed in its own registers before it is added to the running tile (pairwise-style accumulation keeps
+// the float32 error of a 4096-row block near 1e-7 of the diagonal).  The Chan update is the epilogue.
+constexpr int kSyT = 64, kSyK = 16;
+__global__ void __launch_bounds__(256) k_cov_syrk(int C, int D, const float* __restrict__ x, const float* __restrict__ bstats,
+                                                   size_t bstride, float* __restrict__ cov, size_t cstride) {
+  __shared__ __align__(16) float As[kSyK][kSyT];
+  __shared__ __align__(16) float Bs[kSyK][kSyT];
+  __shared__ float mu_i[kSyT], mu_j[kSyT];
+  // lower-triangular tile index -> (ti, tj), ti >= tj
+  const int p = blockIdx.x;
+  int ti = (int)((sqrtf(8.f * (float)p + 1.f) - 1.f) * 0.5f);
+  while (ti * (ti + 1) / 2 > p) --ti;
+  while ((ti + 1) * (ti + 2) / 2 <= p) ++ti;
+  const int tj = p - ti * (ti + 1) / 2;
+  const int b = blockIdx.y;
+  const int c0 = b * kStatBlock, c1 = min(C, c0 + kStatBlock);
+  const float* mu = bstats + (size_t)b * bstride + 2;  // k_block_stats record: (sum accept, n, mean[D], M2[D])
+  float* blk = cov + (size_t)b * cstride;              // (count, -, mean[D], m2[D*D])
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int i0 = ti * kSyT, j0 = tj * kSyT;
+  if (tid < kSyT) {
+    mu_i[tid] = (i0 + tid < D) ? mu[i0 + tid] : 0.f;
+    mu_j[tid] = (j0 + tid < D) ? mu[j0 + tid] : 0.f;
+  }
+  __syncthreads();
+  float acc[4][4], part[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) acc[r][s] = 0.f;
+  const int lc = tid & 63, lk = tid >> 6;
+  const bool iok = i0 + lc < D, jok = j0 + lc < D;
+  for (int k0 = c0; k0 < c1; k0 += kSyK) {
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int k = lk + 4 * r, c = k0 + k;
+      const bool cok = c < c1;
+      As[k][lc] = (cok && iok) ? x[(size_t)c * D + i0 + lc] - mu_i[lc] : 0.f;
+      Bs[k][lc] = (cok && jok) ? x[(size_t)c * D + j0 + lc] - mu_j[lc] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) part[r][s] = 0.f;
+#pragma unroll
+    for (int k = 0; k < kSyK; ++k) {
+      const float4 a = *reinterpret_cast<const float4*>(&As[k][ty * 4]);
+      const float4 bb = *reinterpret_cast<const float4*>(&Bs[k][tx * 4]);
+      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) part[r][s] = fmaf(av[r], bv[s], part[r][s]);
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) acc[r][s] += part[r][s];
+    __syncthreads();
+  }
+  // epilogue: Chan update against the block's accumulated mean (read before k_cov_mean_update rewrites it)
+  float fm, fc, nab;
+  cgl_factors(blk[0], (float)(c1 - c0), fm, fc, nab);
+  const float* am = blk + 2;
+  float* m2 = blk + 2 + D;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int i = i0 + ty * 4 + r;
+    if (i >= D) continue;
+    const float di = mu_i[ty * 4 + r] - am[i];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int j = j0 + tx * 4 + s;
+      if (j > i || j >= D) continue;
+      const float dj = mu_j[tx * 4 + s] - am[j];
+      const size_t o = (size_t)i * D + j;
+      m2[o] = (m2[o] + acc[r][s]) + di * dj * fc;
+    }
+  }
+}
+// count and mean of every block accumulator after the SYRK (one CTA per block: the count is read before it is rewritten)
+__global__ void k_cov_mean_update(int C, int D, const float* __restrict__ bstats, size_t bstride, float* __restrict__ cov, size_t cstride) {
+  const int b = blockIdx.x;
+  const int c0 = b * kStatBlock, c1 = min(C, c0 + kStatBlock);
+  float* blk = cov + (size_t)b * cstride;
+  const float* mu = bstats + (size_t)b * bstride + 2;
+  float fm, fc, nab;
+  cgl_factors(blk[0], (float)(c1 - c0), fm, fc, nab);
+  for (int d = threadIdx.x; d < D; d += blockDim.x) blk[2 + d] = blk[2 + d] + (mu[d] - blk[2 + d]) * fm;
+  __syncthreads();
+  if (threadIdx.x == 0) blk[0] = nab;
+}
+
+// merge the block accumulators in global order and whiten (_recompute_eig_state, :169-189):
+// W = (m2 / max(count - 1, 1)) * s_i * s_j with s = 1 / sqrt(imm).  One thread per lower-triangle element, both halves written.
+__global__ void k_cov_merge_whiten(int D, int nblk, const float* __restrict__ cov, size_t cstride, const float* __restrict__ imm,
+                                   float* __restrict__ W, float* __restrict__ mean_out) {
+  const int i = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j > i) return;
+  float n = 0.f, mi = 0.f, mj = 0.f, m2 = 0.f;
+  for (int b = 0; b < nblk; ++b) {
+    const float* blk = cov + (size_t)b * cstride;
+    if (blk[0] == 0.f) continue;  // an empty block leaves the merge unchanged (cgl_merge_two's n_ab = 0 guard)
+    float fm, fc, nab;
+    cgl_factors(n, blk[0], fm, fc, nab);
+    const float di = blk[2 + i] - mi, dj = blk[2 + j] - mj;
+    m2 = m2 + blk[2 + D + (size_t)i * D + j] + di * dj * fc;
+    mi = mi + di * fm;
+    mj = mj + dj * fm;
+    n = nab;
+  }
+  if (mean_out && j == 0) { mean_out[0] = n; mean_out[1 + i] = mi; }
+  const float cv = m2 / fmaxf(n - 1.f, 1.f);
+  if (imm) {
+    const float w = cv * (1.0f / sqrtf(imm[i])) * (1.0f / sqrtf(imm[j]));
+    W[(size_t)i * D + j] = w;
+    W[(size_t)j * D + i] = w;
+  } else {
+    W[(size_t)i * D + j] = cv;
+    W[(size_t)j * D + i] = cv;
+  }
+}
+
+// one power iteration (_power_iteration_lambda_max, :147-166): v = x / ||x|| (norm guarded to 1 when 0; skipped for the
+// warm start, which is already normalised), y = W v.  Every CTA forms v itself in a fixed order; CTA 0 stores it in v_out.
+// 8 warps per CTA, one row per warp.
+__global__ void __launch_bounds__(256) k_pow_iter(int D, const float* __restrict__ W, const float* __restrict__ x, int normalize,
+                                                  float* __restrict__ v_out, float* __restrict__ y) {
+  __shared__ float v[1024];
+  __shared__ float red[8];
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  float nrm = 1.f;
+  if (normalize) {
+    float s = 0.f;
+    for (int d = tid; d < D; d += 256) s = fmaf(x[d], x[d], s);
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    if (lane == 0) red[w] = s;
+    __syncthreads();
+    float t = 0.f;
+    for (int k = 0; k < 8; ++k) t += red[k];
+    nrm = sqrtf(t);
+    if (!(nrm > 0.f)) nrm = 1.f;
+  }
+  for (int d = tid; d < D; d += 256) v[d] = normalize ? x[d] / nrm : x[d];
+  __syncthreads();
+  if (v_out && blockIdx.x == 0)
+    for (int d = tid; d < D; d += 256) v_out[d] = v[d];
+  const int r = blockIdx.x * 8 + w;
+  if (r >= D) return;
+  float a = 0.f;
+  for (int d = lane; d < D; d += 32) a = fmaf(W[(size_t)r * D + d], v[d], a);
+  for (int off = 16; off > 0; off >>= 1) a += __shfl_xor_sync(0xffffffffu, a, off);
+  if (lane == 0) y[r] = a;
+}
+// lambda_max = max(v . W v, 1e-6) (_LENGTH_FLOOR_LAMBDA_EPS)
+__global__ void k_pow_rayleigh(int D, const float* __restrict__ v, const float* __restrict__ y, float* __restrict__ ms) {
+  __shared__ float red[8];
+  const int tid = threadIdx.x;
+  float s = 0.f;
+  for (int d = tid; d < D; d += 256) s = fmaf(v[d], y[d], s);
+  for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+  if ((tid & 31) == 0) red[tid >> 5] = s;
+  __syncthreads();
+  if (tid == 0) {
+    float t = 0.f;
+    for (int k = 0; k < 8; ++k) t += red[k];
+    ms[MM_LAMBDA] = fmaxf(t, 1e-6f);
+  }
+}
+
+// the metric the next transition uses (_diagonal_mass_matrix_or_fallback, :75-90): max(m2 / (n - 1), 1e-20) once
+// n >= max(64, int(2 sqrt(D))), ones before that
+__global__ void k_mm_imm(int D, float* __restrict__ ms, float* __restrict__ imm) {
+  const double n = (double)ms[MM_WSTEPS] * (double)ms[MM_CG];
+  const bool engaged = n >= (double)ms[MM_THRESH];
+  const float nm1 = (float)(n - 1.0);
+  for (int d = threadIdx.x; d < D; d += blockDim.x) imm[d] = engaged ? fmaxf(ms[kMmHdr + D + d] / nm1, 1e-20f) : 1.f;
+  __syncthreads();
+  if (threadIdx.x == 0) ms[MM_ENGAGED] = engaged ? 1.f : 0.f;
+}
+__global__ void k_mm_init(int D, float* __restrict__ ms, float c_global, float thresh, int whiten, int floor_on, float* __restrict__ imm) {
+  float* eig = ms + kMmHdr + 2 * (size_t)D;
+  const float v0 = 1.0f / sqrtf((float)D);  // ones(D) / sqrt(D) (_eig_state_init, :142-144)
+  for (int d = threadIdx.x; d < D; d += blockDim.x) { imm[d] = 1.f; eig[d] = v0; }
+  if (threadIdx.x == 0) {
+    ms[MM_CG] = c_global; ms[MM_THRESH] = thresh; ms[MM_LAMBDA] = 1.f;
+    ms[MM_WHITEN] = (float)whiten; ms[MM_FLOOR] = (float)floor_on;
+  }
 }
 }  // namespace bjx
 
@@ -628,4 +921,241 @@ extern "C" int bjx_chees_final(bjx_handle_t h, const float* state, float* out2) 
   out2[0] = expf(hst[CH_LOG_EPS_MA]);                       // step_size
   out2[1] = expf(hst[CH_LOG_T_MA] - hst[CH_LOG_EPS_MA]);    // num_leapfrog_steps (integration_steps_params)
   return 0;
+}
+
+// =====================================================================================================================
+// ChEES with mass_matrix_estimation="diagonal" (chees_adaptation.py:61-237,797-1001).  The metric state holds the diagonal
+// accumulator, the power-iteration vectors, this step's payload for the first all-gather (the pass-1 blocks followed by the
+// k_block_stats blocks of the new positions, so an ordinary step adds no collective) and, with the length floor, the
+// per-block covariance accumulators and the whitened matrix of the last recompute.  Only recompute steps (every 32
+// in-window steps, and the final parameters) move D x D data between GPUs: the block accumulators are all-gathered and
+// merged in global block order on every rank (DESIGN.md section 7).
+// =====================================================================================================================
+namespace {
+struct MmLayout {
+  int nb;
+  size_t S1, Sm, R, Sc;                                          // record strides; R = payload floats per rank
+  size_t eig, u0, u1, pay_loc, W, cov_loc, pay_gat, cov_gat, total;
+};
+MmLayout mm_layout(int C, int D, int n_ranks, int options) {
+  MmLayout L{};
+  const size_t d = (size_t)D;
+  const bool fl = options & BJX_CHEES_LENGTH_FLOOR;
+  L.nb = n_stat_blocks(C);
+  L.S1 = 3 + 3 * d;
+  L.Sm = 2 + 2 * d;
+  L.R = (size_t)L.nb * (L.S1 + L.Sm);
+  L.Sc = 2 + d + d * d;
+  size_t o = kMmHdr + 2 * d;                                     // header, accumulator mean[D], m2[D]
+  L.eig = o; o += d;
+  L.u0 = o; o += d;
+  L.u1 = o; o += d;
+  L.pay_loc = o; o += L.R;
+  L.W = o; o += fl ? d * d : 0;
+  L.cov_loc = o; o += fl ? (size_t)L.nb * L.Sc : 0;
+  L.pay_gat = o; o += n_ranks > 1 ? L.R * n_ranks : 0;
+  L.cov_gat = o; o += (fl && n_ranks > 1) ? (size_t)L.nb * L.Sc * n_ranks : 0;
+  L.total = o;
+  return L;
+}
+
+// fold new positions q [C, D] into the block covariance accumulators; their k_block_stats records are at stats
+int cov_fold(bjx_handle_t h, const MmLayout& L, float* ms, const float* q, const float* stats) {
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  const int tiles = (D + kSyT - 1) / kSyT;
+  k_cov_syrk<<<dim3(tiles * (tiles + 1) / 2, L.nb), 256, 0, h->stream>>>(C, D, q, stats, L.Sm, ms + L.cov_loc, L.Sc);
+  BJX_CHECK_LAUNCH("k_cov_syrk");
+  k_cov_mean_update<<<L.nb, 256, 0, h->stream>>>(C, D, stats, L.Sm, ms + L.cov_loc, L.Sc);
+  BJX_CHECK_LAUNCH("k_cov_mean_update");
+  return 0;
+}
+
+// merged block accumulators -> W (whitened by imm, or the plain covariance with imm = NULL); block order is global
+int cov_merge(bjx_handle_t h, void* comm, int n_ranks, const MmLayout& L, float* ms, const float* imm, float* W, float* mean_out) {
+  const int D = h->cfg.dim;
+  const float* cov = ms + L.cov_loc;
+  if (n_ranks > 1) {
+    int rc = bjx_allgather_stats(h, comm, ms + L.cov_loc, (int64_t)(L.nb * L.Sc), ms + L.cov_gat);
+    if (rc) return rc;
+    cov = ms + L.cov_gat;
+  }
+  k_cov_merge_whiten<<<dim3((D + 255) / 256, D), 256, 0, h->stream>>>(D, L.nb * n_ranks, cov, L.Sc, imm, W, mean_out);
+  BJX_CHECK_LAUNCH("k_cov_merge_whiten");
+  return 0;
+}
+
+// _recompute_eig_state: whiten by imm, `iters` power iterations warm-started from the stored eigenvector, lambda_max
+int mm_recompute(bjx_handle_t h, void* comm, int n_ranks, const MmLayout& L, float* ms, const float* imm, int iters) {
+  const int D = h->cfg.dim;
+  int rc = cov_merge(h, comm, n_ranks, L, ms, imm, ms + L.W, nullptr);
+  if (rc) return rc;
+  const float* W = ms + L.W;
+  float* u[2] = {ms + L.u0, ms + L.u1};
+  const int g = (D + 7) / 8;
+  k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, ms + L.eig, 0, nullptr, u[0]);
+  for (int k = 1; k < iters; ++k) k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, u[(k - 1) & 1], 1, nullptr, u[k & 1]);
+  k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, u[(iters - 1) & 1], 1, ms + L.eig, u[iters & 1]);
+  k_pow_rayleigh<<<1, 256, 0, h->stream>>>(D, ms + L.eig, u[iters & 1], ms);
+  BJX_CHECK_LAUNCH("k_pow_iter");
+  return 0;
+}
+
+constexpr int kFloorIters = 5, kFloorFinalIters = 20;  // chees_adaptation.py:121-122 (the 32-step cadence is the caller's)
+}  // namespace
+
+extern "C" int64_t bjx_chees_metric_state_floats(int32_t n_chains_local, int32_t dim, int32_t n_ranks, int32_t options) {
+  if (n_chains_local <= 0 || dim <= 0 || dim > 1024 || n_ranks <= 0) return 0;
+  return (int64_t)mm_layout(n_chains_local, dim, n_ranks, options).total;
+}
+
+extern "C" int bjx_chees_metric_init(bjx_handle_t h, float* metric_state, int32_t n_ranks, int32_t options, float* imm_out) {
+  if (!h || !metric_state || !imm_out) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (n_ranks < 1 || (options & ~(BJX_CHEES_WHITEN | BJX_CHEES_LENGTH_FLOOR))) return bjx_fail(h, BJX_E_INVALID, "bad n_ranks / options");
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const MmLayout L = mm_layout(C, D, n_ranks, options);
+  BJX_CUDA(cudaMemsetAsync(metric_state, 0, L.total * sizeof(float), h->stream));
+  const int thresh = std::max(64, (int)(2.0 * std::sqrt((double)D)));  // _mass_matrix_engagement_threshold, :61-72
+  k_mm_init<<<1, 256, 0, h->stream>>>(D, metric_state, (float)((double)C * n_ranks), (float)thresh,
+                                       (options & BJX_CHEES_WHITEN) ? 1 : 0, (options & BJX_CHEES_LENGTH_FLOOR) ? 1 : 0, imm_out);
+  BJX_CHECK_LAUNCH("k_mm_init");
+  return bjx_set_metric(h, BJX_METRIC_DIAG, imm_out);
+}
+
+extern "C" int bjx_chees_update_metric(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, float* state,
+                                       float* metric_state, const float* initial_position, const float* proposal_position,
+                                       const float* proposal_momentum, const float* new_position, const float* acceptance_rate,
+                                       const uint8_t* is_divergent, float learning_rate, float b1, float b2,
+                                       float target_acceptance, float decay_rate, int32_t max_leapfrog_steps, int32_t in_window,
+                                       int32_t recompute, float* step_size_chain, int32_t* steps_chain, float* history,
+                                       float* imm, float* lambda_history, float* engaged_history) {
+  if (!h || !state || !metric_state || !initial_position || !proposal_position || !proposal_momentum || !new_position ||
+      !acceptance_rate || !is_divergent || !step_size_chain || !steps_chain || !imm)
+    return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
+  const bool floor_on = options & BJX_CHEES_LENGTH_FLOOR;
+  if (recompute && !(in_window && floor_on))
+    return bjx_fail(h, BJX_E_INVALID, "recompute needs an in-window step and the length floor");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  const MmLayout L = mm_layout(C, D, n_ranks, options);
+  const int nb = L.nb;
+  float* ms = metric_state;
+  float* w = state + kChHdr + 2 * (size_t)D;
+  float* num = w + C;
+  float* den = num + C;
+  float* loc2 = den + C + (size_t)nb * L.S1 * (1 + n_ranks);  // the pass-2 regions of the identity-metric layout
+  float* gat2 = loc2 + (size_t)nb * 2;
+  float* loc1 = ms + L.pay_loc;
+  float* locm = loc1 + (size_t)nb * L.S1;                     // k_block_stats records of the new positions
+  cudaStream_t s = h->stream;
+  k_chees_w<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, acceptance_rate, is_divergent, w);
+  k_chees_pass1<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, proposal_position, initial_position, acceptance_rate,
+                                                              is_divergent, w, loc1);
+  BJX_CHECK_LAUNCH("k_chees_pass1");
+  if (in_window) {
+    k_block_stats<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, new_position, acceptance_rate, locm);
+    BJX_CHECK_LAUNCH("k_block_stats");
+  }
+  const float* m1 = loc1;
+  if (n_ranks > 1) {
+    int rc = bjx_allgather_stats(h, nccl_comm, loc1, (int64_t)L.R, ms + L.pay_gat);
+    if (rc) return rc;
+    m1 = ms + L.pay_gat;
+  }
+  k_chees_means_metric<<<1, 512, 0, s>>>(D, nb * n_ranks, m1, state, nb, L.R, ms, in_window);
+  if (options & BJX_CHEES_WHITEN)  // the criterion of this step uses the metric of this step's transition
+    k_chees_dots<true><<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, proposal_momentum, initial_position, acceptance_rate,
+                                                   is_divergent, state, num, den, imm);
+  else
+    k_chees_dots<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, proposal_momentum, initial_position, acceptance_rate,
+                                             is_divergent, state, num, den);
+  k_chees_pass2<<<nb, 256, 0, s>>>(C, num, den, loc2);
+  BJX_CHECK_LAUNCH("k_chees_pass2");
+  const float* m2 = loc2;
+  if (n_ranks > 1) {
+    int rc = bjx_allgather_stats(h, nccl_comm, loc2, (int64_t)(nb * 2), gat2);
+    if (rc) return rc;
+    m2 = gat2;
+  }
+  if (in_window && floor_on) {
+    int rc = cov_fold(h, L, ms, new_position, locm);
+    if (rc) return rc;
+    if (recompute) {  // against the metric this step's transition used, before this step's fold engages (:898-903)
+      rc = mm_recompute(h, nccl_comm, n_ranks, L, ms, imm, kFloorIters);
+      if (rc) return rc;
+    }
+  }
+  if (in_window) {
+    k_mm_imm<<<1, 1024, 0, s>>>(D, ms, imm);
+    BJX_CHECK_LAUNCH("k_mm_imm");
+  }
+  k_chees_finish<true><<<1, 32, 0, s>>>(nb * n_ranks, m2, state, learning_rate, b1, b2, target_acceptance, decay_rate,
+                                        (float)max_leapfrog_steps, history, ms, lambda_history, engaged_history);
+  k_fill_from<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_EPS, step_size_chain);
+  k_fill_steps<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_L, steps_chain);
+  BJX_CHECK_LAUNCH("k_chees_finish");
+  if (in_window) return bjx_set_metric(h, BJX_METRIC_DIAG, imm);  // mass_matrix_sqrt of the new estimate, on the stream
+  return 0;
+}
+
+extern "C" int bjx_chees_final_metric(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, const float* state,
+                                      float* metric_state, int32_t max_leapfrog_steps, const float* imm, float* out4_host) {
+  if (!h || !state || !metric_state || !imm || !out4_host) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  const MmLayout L = mm_layout(C, D, n_ranks, options);
+  if (options & BJX_CHEES_LENGTH_FLOOR) {  // 20 power iterations against the final metric (:971-978)
+    int rc = mm_recompute(h, nccl_comm, n_ranks, L, metric_state, imm, kFloorFinalIters);
+    if (rc) return rc;
+  }
+  float hst[kChHdr], hdr[kMmHdr];
+  BJX_CUDA(cudaMemcpyAsync(hst, state, sizeof(hst), cudaMemcpyDeviceToHost, h->stream));
+  BJX_CUDA(cudaMemcpyAsync(hdr, metric_state, sizeof(hdr), cudaMemcpyDeviceToHost, h->stream));
+  BJX_CUDA(cudaStreamSynchronize(h->stream));
+  // final parameters (:958-1001), on the host as bjx_chees_final forms them
+  const float eps = expf(hst[CH_LOG_EPS_MA]);
+  float n_lf = expf(hst[CH_LOG_T_MA] - hst[CH_LOG_EPS_MA]), clipped = 0.f;
+  if (options & BJX_CHEES_LENGTH_FLOOR) {  // floor re-applied to exp(log T_ma), divided by exp(log eps_ma)
+    const bool engaged = hdr[MM_ENGAGED] != 0.f;
+    const float floor_v = engaged ? 1.57079637f * sqrtf(hdr[MM_LAMBDA]) : 0.f;
+    const float cap = (float)max_leapfrog_steps * eps;
+    n_lf = fminf(fmaxf(expf(hst[CH_LOG_T_MA]), floor_v), cap) / eps;
+    clipped = (engaged && floor_v > cap) ? 1.f : 0.f;
+  }
+  out4_host[0] = eps;
+  out4_host[1] = n_lf;
+  out4_host[2] = clipped;
+  out4_host[3] = hdr[MM_LAMBDA];
+  return 0;
+}
+
+extern "C" int bjx_chees_metric_fold_covariance(bjx_handle_t h, int32_t options, float* metric_state, const float* q) {
+  if (!h || !metric_state || !q) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (!(options & BJX_CHEES_LENGTH_FLOOR)) return bjx_fail(h, BJX_E_INVALID, "the covariance accumulator needs the length floor");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  const MmLayout L = mm_layout(C, D, 1, options);
+  float* locm = metric_state + L.pay_loc + (size_t)L.nb * L.S1;
+  // k_block_stats also sums an acceptance array over each block; q stands in for it (that sum is not read here)
+  k_block_stats<<<dim3((D + 31) / 32, L.nb), dim3(32, 8), 0, h->stream>>>(C, D, q, q, locm);
+  BJX_CHECK_LAUNCH("k_block_stats");
+  return cov_fold(h, L, metric_state, q, locm);
+}
+
+extern "C" int bjx_chees_metric_covariance(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, float* metric_state,
+                                           float* out) {
+  if (!h || !metric_state || !out) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
+  if (!(options & BJX_CHEES_LENGTH_FLOOR)) return bjx_fail(h, BJX_E_INVALID, "the covariance accumulator needs the length floor");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  const MmLayout L = mm_layout(C, D, n_ranks, options);
+  return cov_merge(h, nccl_comm, n_ranks, L, metric_state, nullptr, out + 1 + D, out);
 }

@@ -349,6 +349,40 @@ int bjx_chees_update(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, float* st
  * synchronises the stream */
 int bjx_chees_final(bjx_handle_t h, const float* state, float* out2_host);
 
+/* ---- ChEES with an ensemble-estimated diagonal metric (chees_adaptation.py:61-237,797-1001, mass_matrix_estimation=
+ * "diagonal") ----------------------------------------------------------------------------------------------------------------
+ * Same step as bjx_chees_update plus: in-window steps fold the new positions (after the transition) of all chains of all
+ * ranks into a diagonal accumulator (pooled in BJX_STAT_BLOCK_CHAINS blocks, carried by the step's first all-gather) and
+ * rewrite imm [D] = max(m2 / (n - 1), 1e-20) once n >= max(64, int(2 sqrt(D))), ones before that; the handle's metric is
+ * re-installed on the stream.  options: BJX_CHEES_WHITEN whitens the criterion by imm; BJX_CHEES_LENGTH_FLOOR also keeps a
+ * windowed D x D covariance accumulator per block, refreshes lambda_max (top eigenvalue of the imm-whitened covariance, 5
+ * power iterations) on steps with `recompute`, and the next transition consumes min(max(T, (pi/2) sqrt(lambda_max)),
+ * max_leapfrog_steps * eps) once imm is engaged.  dim <= 1024.  `state` is a bjx_chees_state_floats buffer initialised
+ * by bjx_chees_init, metric_state a bjx_chees_metric_state_floats buffer initialised by bjx_chees_metric_init (which
+ * sets imm_out to ones and installs it).  lambda_history / engaged_history (nullable, device [num_steps]): lambda_max and
+ * the engagement flag after step t, i.e. those the transition of step t + 1 uses. */
+#define BJX_CHEES_WHITEN 1
+#define BJX_CHEES_LENGTH_FLOOR 2
+int64_t bjx_chees_metric_state_floats(int32_t n_chains_local, int32_t dim, int32_t n_ranks, int32_t options);
+int bjx_chees_metric_init(bjx_handle_t h, float* metric_state, int32_t n_ranks, int32_t options, float* imm_out);
+int bjx_chees_update_metric(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, float* state,
+                            float* metric_state, const float* initial_position, const float* proposal_position,
+                            const float* proposal_momentum, const float* new_position, const float* acceptance_rate,
+                            const uint8_t* is_divergent, float learning_rate, float b1, float b2, float target_acceptance,
+                            float decay_rate, int32_t max_leapfrog_steps, int32_t in_window, int32_t recompute,
+                            float* step_size_chain, int32_t* steps_chain, float* history, float* imm, float* lambda_history,
+                            float* engaged_history);
+/* out4 (HOST): step_size, num_leapfrog_steps (with the floor re-applied after 20 power iterations against imm),
+ * floor_clipped_by_cap (0 / 1), lambda_max; synchronises the stream */
+int bjx_chees_final_metric(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, const float* state,
+                           float* metric_state, int32_t max_leapfrog_steps, const float* imm, float* out4_host);
+/* Fold positions q [C, D] (device) into this rank's windowed covariance accumulators, as an in-window step does
+ * (needs BJX_CHEES_LENGTH_FLOOR). */
+int bjx_chees_metric_fold_covariance(bjx_handle_t h, int32_t options, float* metric_state, const float* q);
+/* The accumulators merged over all ranks: out (device) = (count, mean[D], covariance m2 / max(count - 1, 1) [D, D]). */
+int bjx_chees_metric_covariance(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, float* metric_state,
+                                float* out);
+
 /* ---- diagnostics on a device-resident history (SURVEY 8f item 3) ---------------------------------------------- */
 /* blackjax.diagnostics.potential_scale_reduction (diagnostics.py:39-89): history float32 [num_samples, C, D] as written
  * by bjx_hmc_sample; rhat_out float32 [D]; scratch: at least 2*C*D + 4 + 4*D floats (device). */
