@@ -91,7 +91,19 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warp are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulators are written asynchronously: keep the compiler from reading them before the wait that completes them
+__device__ __forceinline__ void fence_operands(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// per-thread register budget of the calling warpgroup (the CTA's total stays within 384 x 168)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // d[64 x 128] += A[64 x 16] . B[128 x 16]^T, both operands K-major in shared memory, float32 accumulators in registers
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
@@ -126,8 +138,11 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t u) { return __half22float2(
 // Tiles t = (t / tiles_n, t % tiles_n) are dealt round-robin over the persistent CTAs; CTAs running side by side share
 // one row block of X (the constant matrix stays L2-resident).
 //   warp 0, lane 0   TMA producer: four tiles per stage into the ring
-//   warpgroups 1-2   consumers: warpgroup w owns rows [64 (w-1), +64) of the tile; per stage 3 x 4 wgmma, then the
-//                    stage is released (one arrival per consumer warp); per tile the epilogue from the registers.
+//   warpgroups 1-2   consumers: warpgroup w owns rows [64 (w-1), +64) of the tile; per stage 3 x 4 wgmma, and once
+//                    they are issued the previous stage's group is waited for and that stage released (one arrival per
+//                    consumer warp); per tile the epilogue from the registers, its global inputs loaded before the
+//                    tile's K loop.  The producer warpgroup runs on 40 registers per thread so that the consumers
+//                    can hold those inputs beside the accumulators (232).
 // Accumulator fragment of m64n128 (per warp of the warpgroup): d[4j + 2h + e] is row 16 warp + 8h + lane / 4,
 // column 8j + 2 (lane % 4) + e.
 __global__ void __launch_bounds__(kThreads, 1)
@@ -159,7 +174,9 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
   if (warp < 4) {
-    // ===== TMA producer
+    // ===== TMA producer.  The whole warpgroup hands its registers to the consumers (which hold the accumulators and
+    // the prefetched epilogue inputs) before warps 1-3 leave.
+    setmaxnreg_dec<40>();
     if (warp == 0 && lane == 0) {
       int s = 0;
       uint32_t ph = 0;
@@ -181,15 +198,45 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
   }
 
   // ===== consumers
+  setmaxnreg_inc<232>();
   const int wg = (warp >> 2) - 1, wq = warp & 3;
   const float mat_unscale = E.mat_unscale ? E.mat_unscale[0] : 1.0f;
   int s = 0;
   uint32_t ph = 0;
   for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     const int m0 = (t / tiles_n) * kBM, n0 = (t % tiles_n) * kBN;
+    // Every input of this tile's epilogue is loaded here, so that the loads complete behind the K loop's MMAs and the
+    // epilogue itself only computes and stores.  Y may alias Cin, but only elementwise: element (r, c) is read as Cin and
+    // written as Y by the same thread and by no other, so reading it before the K loop reads the same value.  The per-row
+    // arrays read here (step sizes, unscales, stale maxima) are never among the same launch's outputs.
+    float al_row[2], sc_row[2];
+    float2 cin[2][kBN / 8];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = m0 + 64 * wg + 16 * wq + 8 * h + (lane >> 2);
+      // per-row epilogue factor and the lift of this row's planes
+      float al = E.alpha, sc = 1.0f;
+      if (r < M) {
+        if (E.alpha_dev) al = E.alpha_dev[r] * E.alpha;
+        al = al * (E.x_unscale ? E.x_unscale[r] : 1.0f) * mat_unscale;
+        if (E.planes) sc = plane_lift(E.stale_max[r]);
+      }
+      al_row[h] = al;
+      sc_row[h] = sc;
+#pragma unroll
+      for (int j = 0; j < kBN / 8; ++j) {
+        const int c = n0 + 8 * j + 2 * (lane & 3);
+        cin[h][j] = make_float2(0.f, 0.f);
+        if (E.has_cin && r < M && c < N) cin[h][j] = *reinterpret_cast<const float2*>(Cin + (size_t)r * N + c);
+      }
+    }
+
+    // One wgmma group stays in flight: K block kb's MMAs are issued before the wait for block kb - 1's, whose stage is
+    // released only then.  wgmmas on one accumulator complete in issue order, so the sums are those of a serial loop.
     float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int s_prev = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       mbar_wait(full_bar(s), ph);
       const uint32_t st = base + (uint32_t)s * kStageBytes;
@@ -204,26 +251,27 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
 #pragma unroll
       for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx1 + 2u * k, da2 + 2u * k);
       wgmma_commit();
-      wgmma_wait_all();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(s));
+      wgmma_wait<1>();
+      if (kb > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar(s_prev));
+      }
+      s_prev = s;
       if (++s == kStages) { s = 0; ph ^= 1u; }
     }
+    wgmma_wait<0>();
+    fence_operands(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_bar(s_prev));
 
     // epilogue: two rows per thread, two adjacent columns per fragment register pair
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = m0 + 64 * wg + 16 * wq + 8 * h + (lane >> 2);
       const bool live = r < M;
-      // per-row epilogue factor and the lift of this row's planes
-      float al = E.alpha, sc = 1.0f, amax = 0.f;
-      if (live) {
-        if (E.alpha_dev) al = E.alpha_dev[r] * E.alpha;
-        al = al * (E.x_unscale ? E.x_unscale[r] : 1.0f) * mat_unscale;
-        if (E.planes) sc = plane_lift(E.stale_max[r]);
-      }
+      const float al = al_row[h], sc = sc_row[h];
+      float amax = 0.f;
       float* yr = Y + (size_t)r * N;
-      const float* cr = Cin ? Cin + (size_t)r * N : nullptr;
       uint16_t* pr = planes_out ? planes_out + (size_t)r * 2 * KP_out : nullptr;
 #pragma unroll
       for (int j = 0; j < kBN / 8; ++j) {
@@ -232,7 +280,7 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
         const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
         float2 y;
         if (E.has_cin) {
-          const float2 cv = *reinterpret_cast<const float2*>(cr + c);
+          const float2 cv = cin[h][j];
           if (E.double_kick) {
             y.x = fmaf(al, a0, fmaf(al, a0, cv.x));
             y.y = fmaf(al, a1, fmaf(al, a1, cv.y));
