@@ -6,15 +6,22 @@ Mirrors ``blackjax.meads_adaptation`` (blackjax/adaptation/meads_adaptation.py:3
 nothing read back), one ``bjx_ghmc_step`` of every chain with its fold's parameters (fold ``t mod K`` frozen), and every
 K steps ``bjx_permutation`` + ``bjx_gather_rows`` (``jax.random.permutation`` of all chains).  The loop never
 synchronises with the host.
+
+With ``low_rank_rank=k`` (MEADS-LRD, :459-784) every chain samples with ONE low-rank metric per step instead of the fold
+scales: ``bjx_meads_lrd_update`` replaces ``bjx_meads_update`` (it also folds the positions into the windowed covariance
+accumulator, runs the on-device eigensolver and rewrites the handle's low-rank metric in place), and the run returns a
+``LowRankMetric`` as ``momentum_inverse_scale``.  Built for dim <= 512 and k <= 16 on one GPU.
 """
+import warnings
 from typing import NamedTuple
 
 import torch
 
 from .. import random as bjx_random
-from .._lib import check, lib, ptr
+from .._lib import BjxError, check, lib, ptr
 from ..base import AdaptationAlgorithm, AdaptationResults
 from ..mcmc import ghmc
+from ..mcmc.metrics import LowRankMetric
 
 __all__ = ["MEADSAdaptationState", "base", "maximum_eigenvalue", "meads_adaptation"]
 
@@ -50,6 +57,67 @@ class _Folds:
 
     def snapshot(self, t):
         return MEADSAdaptationState(t, self.step_size.clone(), self.sigma.clone(), self.alpha.clone(), self.delta.clone())
+
+
+class _LowRank:
+    """Device buffers of bjx_meads_lrd_update / bjx_meads_lrd_metric for (C chains, D dims, rank k, K folds).  The
+    handle must hold a rank-k low-rank metric; ``install`` puts the fallback one there."""
+
+    MAX_DIM, MAX_RANK = 512, 16
+    ENGAGED, ITERS, RESID, NOCONV, ITERS_SUM, ITERS_MAX, SOLVES = range(7)   # header slots (include/bjx.h)
+
+    def __init__(self, eng, k, K):
+        L = lib()
+        self.eng, self.k, self.K = eng, k, K
+        dev, C, D = eng.device, eng.C, eng.D
+        self.state = torch.zeros(L.bjx_meads_lrd_state_floats(C, D, k), dtype=torch.float32, device=dev)
+        self.scratch = torch.empty(L.bjx_meads_lrd_scratch_floats(C, D, K), dtype=torch.float32, device=dev)
+        self.header = self.state[:16]
+        o = 16
+        self.sigma = self.state[o:o + D]
+        self.U = self.state[o + D:o + D + D * k].view(D, k)
+        self.lam = self.state[o + D + D * k:o + D + D * k + k]
+
+    def install(self):
+        """The fallback metric (ones, eye(D, k), ones); each update rewrites it in place."""
+        D, k, dev = self.eng.D, self.k, self.eng.device
+        metric = LowRankMetric(torch.ones(D, device=dev), torch.eye(D, k, device=dev), torch.ones(k, device=dev))
+        try:
+            self.eng.ensure_metric(metric)
+        except BjxError as e:
+            raise NotImplementedError(f"meads_adaptation(low_rank_rank=...) needs a target whose transitions run on the "
+                                      f"warp kernels with a low-rank metric: {e}") from None
+
+    def update(self, folds, q, g, t, in_window, multiplier, slowdown):
+        check(lib().bjx_meads_lrd_update(self.eng.h, ptr(q), ptr(g), self.K, int(t), int(bool(in_window)), float(multiplier),
+                                         float(slowdown), ptr(folds.state), ptr(self.state), ptr(self.scratch)), self.eng.h)
+
+    def metric(self, final_q):
+        """The final parameters (:746-771) as a LowRankMetric of new device tensors."""
+        D, k, dev = self.eng.D, self.k, self.eng.device
+        sigma, U, lam = (torch.empty(s, dtype=torch.float32, device=dev) for s in ((D,), (D, k), (k,)))
+        check(lib().bjx_meads_lrd_metric(self.eng.h, ptr(self.state), ptr(final_q), ptr(sigma), ptr(U), ptr(lam)), self.eng.h)
+        return LowRankMetric(sigma, U, lam)
+
+    def warn_if_not_converged(self):
+        """One host read of the eigensolver's diagnostics, after the run: warn when any solve stopped at its cap."""
+        h = self.header.cpu().tolist()
+        if h[self.NOCONV]:
+            solves = max(h[self.SOLVES], 1.0)
+            warnings.warn(f"MEADS-LRD: the eigensolver stopped at its iteration cap in at least one of {int(h[self.SOLVES])} "
+                          f"solves (mean {h[self.ITERS_SUM] / solves:.1f}, max {int(h[self.ITERS_MAX])} iterations; last "
+                          f"relative residual {h[self.RESID]:.2e}); the low-rank metric may be inaccurate", RuntimeWarning,
+                          stacklevel=3)
+
+
+def _low_rank_limits(logdensity_fn, k, D):
+    """This port's limits of MEADS-LRD (NotImplementedError), after the rank is clamped to D."""
+    if D > _LowRank.MAX_DIM or k > _LowRank.MAX_RANK:
+        raise NotImplementedError(f"meads_adaptation(low_rank_rank=...) is built for dim <= {_LowRank.MAX_DIM} and a rank "
+                                  f"<= {_LowRank.MAX_RANK}; got dim {D}, rank {k}")
+    if not getattr(logdensity_fn, "build_options", {}).get("dense_metric", True):
+        raise NotImplementedError("meads_adaptation(low_rank_rank=...) needs the low-rank metric kernels: build the "
+                                  "UserTarget with dense_metric=True")
 
 
 def _engine_for(positions, logdensity_fn):
@@ -112,15 +180,24 @@ def _scratch_engine(x):
 def meads_adaptation(logdensity_fn, num_chains: int, num_folds: int = 4, step_size_multiplier: float = 0.5,
                      damping_slowdown: float = 1.0, adaptation_info_fn=None, low_rank_rank=None,
                      low_rank_window_fraction: float = 0.5):
-    """meads_adaptation.py:316-784 (``low_rank_rank=None``).  ``run(rng_key, positions, num_steps)`` returns
-    ``(AdaptationResults(last GHMCState, parameters), info)``; ``info`` is the list of what ``adaptation_info_fn(state,
-    info, adaptation_state)`` returned per step (None: nothing is stored)."""
+    """meads_adaptation.py:316-784.  ``run(rng_key, positions, num_steps)`` returns ``(AdaptationResults(last GHMCState,
+    parameters), info)``; ``info`` is the list of what ``adaptation_info_fn(state, info, adaptation_state)`` returned per
+    step (None: nothing is stored).  ``low_rank_rank=k`` adapts one rank-min(k, num_chains - 1, dim) low-rank metric
+    for all chains (MEADS-LRD), estimated from the covariance of all chains' positions over the last
+    ``low_rank_window_fraction`` of the steps; ``parameters["momentum_inverse_scale"]`` is then a ``LowRankMetric``."""
     if num_folds < 1:
         raise ValueError(f"num_folds must be >= 1, got {num_folds}.")
     if num_chains % num_folds != 0:
         raise ValueError(f"num_chains ({num_chains}) must be divisible by num_folds ({num_folds}).")
-    if low_rank_rank is not None:
-        raise NotImplementedError("meads_adaptation is built for low_rank_rank=None (diagonal momentum scale per fold)")
+    low_rank_k = None
+    if low_rank_rank is not None:                                # :467-487
+        low_rank_k = min(int(low_rank_rank), num_chains - 1)
+        if low_rank_k < 1:
+            raise ValueError(f"low_rank_rank={low_rank_rank} cannot be honored: the low-rank metric is estimated from "
+                             f"the full population of num_chains={num_chains} chains, and that estimate needs "
+                             "num_chains - 1 >= 1. Increase num_chains.")
+        if not 0.0 <= low_rank_window_fraction <= 1.0:
+            raise ValueError(f"low_rank_window_fraction must be in [0.0, 1.0], got {low_rank_window_fraction}.")
     n_per_fold = num_chains // num_folds
     kernel = ghmc.build_kernel(inplace=True)
 
@@ -130,7 +207,13 @@ def meads_adaptation(logdensity_fn, num_chains: int, num_folds: int = 4, step_si
         if C != num_chains:
             raise ValueError("initial `positions` leading dimension must be equal to the `num_chains`")
         dev = positions.device
+        lowrank = None
+        if low_rank_k is not None:
+            _low_rank_limits(logdensity_fn, min(low_rank_k, D), D)
         eng = _engine_for(positions, logdensity_fn)
+        if low_rank_k is not None:
+            lowrank = _LowRank(eng, min(low_rank_k, D), num_folds)
+            lowrank.install()
         L = lib()
         k2 = bjx_random.split(rng_key.to(dev), 2).view(torch.int32)
         key_init, key_adapt = k2[0].contiguous(), k2[1].contiguous()
@@ -146,12 +229,18 @@ def meads_adaptation(logdensity_fn, num_chains: int, num_folds: int = 4, step_si
         spare = tuple(torch.empty_like(x) for x in state)
         perm = torch.empty(C, dtype=torch.int32, device=dev)
         perm_scratch = torch.empty(L.bjx_permutation_scratch_bytes(C), dtype=torch.uint8, device=dev)
+        window_start = int(low_rank_window_fraction * num_steps)    # :723
         infos = []
         for t in range(num_steps):
-            folds.update(state.position, state.logdensity_grad, t, step_size_multiplier, damping_slowdown)
             skip = ((t % num_folds) * n_per_fold, (t % num_folds + 1) * n_per_fold) if num_folds > 1 else (0, 0)
-            state, info = kernel(keys[t], state, logdensity_fn, None, None, None, None,
-                                 _rows=(folds.step_size, folds.alpha, folds.delta, folds.imm, folds.msqrt, n_per_fold, skip))
+            if lowrank is None:
+                folds.update(state.position, state.logdensity_grad, t, step_size_multiplier, damping_slowdown)
+                rows = (folds.step_size, folds.alpha, folds.delta, folds.imm, folds.msqrt, n_per_fold, skip)
+            else:                                                # one shared metric, in the handle (:549-568,644-667)
+                lowrank.update(folds, state.position, state.logdensity_grad, t, t >= window_start, step_size_multiplier,
+                               damping_slowdown)
+                rows = (folds.step_size, folds.alpha, folds.delta, None, None, n_per_fold, skip)
+            state, info = kernel(keys[t], state, logdensity_fn, None, None, None, None, _rows=rows)
             if num_folds > 1 and (t + 1) % num_folds == 0:     # shuffle_key = split(rng_key, C + 1)[C]  (:503-504,675-683)
                 check(L.bjx_permutation(eng.h, ptr(keys[t]), C, C, ptr(perm), ptr(perm_scratch)), eng.h)
                 for src, dst in zip(state, spare):
@@ -163,10 +252,13 @@ def meads_adaptation(logdensity_fn, num_chains: int, num_folds: int = 4, step_si
         last = folds.snapshot(num_steps)
         parameters = {
             "step_size": last.step_size.mean(),
-            "momentum_inverse_scale": last.position_sigma.mean(dim=0),
+            "momentum_inverse_scale": (last.position_sigma.mean(dim=0) if lowrank is None
+                                       else lowrank.metric(state[0].contiguous())),
             "alpha": last.alpha.mean(),
             "delta": last.delta.mean(),
         }
+        if lowrank is not None:
+            lowrank.warn_if_not_converged()
         return AdaptationResults(ghmc.GHMCState(*state), parameters), infos
 
     return AdaptationAlgorithm(run)

@@ -840,6 +840,22 @@ __global__ void k_mm_init(int D, float* __restrict__ ms, float c_global, float t
     ms[MM_WHITEN] = (float)whiten; ms[MM_FLOOR] = (float)floor_on;
   }
 }
+
+// The block covariance accumulators on their own, for MEADS-LRD (bjx_meads.cu); the same kernels and block order as above.
+int cov_stat_blocks(int C) { return n_stat_blocks(C); }
+size_t cov_block_floats(int D) { return 2 + (size_t)D + (size_t)D * D; }
+void launch_cov_fold(int C, int D, const float* q, float* stats, float* cov, cudaStream_t s) {
+  const int nb = n_stat_blocks(C), tiles = (D + kSyT - 1) / kSyT;
+  const size_t sstride = 2 + 2 * (size_t)D;
+  // k_block_stats also sums an acceptance array over each block; q stands in for it (that sum is not read here)
+  k_block_stats<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, q, q, stats);
+  k_cov_syrk<<<dim3(tiles * (tiles + 1) / 2, nb), 256, 0, s>>>(C, D, q, stats, sstride, cov, cov_block_floats(D));
+  k_cov_mean_update<<<nb, 256, 0, s>>>(C, D, stats, sstride, cov, cov_block_floats(D));
+}
+void launch_cov_merge(int C, int D, const float* cov, float* out, float* count_mean, cudaStream_t s) {
+  k_cov_merge_whiten<<<dim3((D + 255) / 256, D), 256, 0, s>>>(D, n_stat_blocks(C), cov, cov_block_floats(D), nullptr, out,
+                                                             count_mean);
+}
 }  // namespace bjx
 
 extern "C" int64_t bjx_chees_state_floats(int32_t n_chains_local, int32_t dim, int32_t n_ranks) {

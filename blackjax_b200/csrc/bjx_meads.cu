@@ -14,8 +14,11 @@
 // jax.random.permutation for the shuffle every K steps (:675-683) is JAX's sort-based shuffle (jax/_src/random.py
 // _shuffle: ceil(3 ln n / ln(2^32-1)) rounds of a stable sort by 32 fresh random bits): a bitonic sort of the 64-bit
 // composites (bits << 32 | position), which orders ties by position exactly like a stable sort.
+#include <cooperative_groups.h>
+
 #include <algorithm>
 #include <cmath>
+#include <mutex>
 
 #include "bjx_handle.h"
 #include "bjx_internal.h"
@@ -285,6 +288,468 @@ static int meads_pairs(int D) {
   const int T = (D + 31) / 32;
   return T * (T + 1) / 2;
 }
+
+// ---- MEADS-LRD (meads_adaptation.py:459-784 with low_rank_rank = k) -----------------------------------------------
+// One low-rank metric (sigma, U, lam) for all chains per warm-up step.  In the window the positions of all chains are
+// folded into the windowed covariance accumulators of bjx_adapt.cu (cgl_update_batch); once they hold 2 D samples the
+// metric is the top-k eigenpairs by |lam - 1| of the pooled correlation matrix R (sample_covariance_eigh_low_rank,
+// metric_estimators.py:543-615), else the diagonal fallback sigma = std of all positions, U = eye(D, k), lam = 1
+// (:263-289).  lam is floored at 1e-6 (:292-313).
+//
+// Eigensolver (k_lrd_eig): the top-k by |lam - 1| of R span the dominant-|mu| invariant subspace of A = R - I.  One
+// cluster of 8 CTAs holds A row-partitioned in shared memory (D <= 512: at most 64 rows of 513 floats per CTA) and runs
+// block orthogonal iteration with b = min(D, 2k + 16) columns: Y = A V, with V read slice by slice from the other CTAs
+// through distributed shared memory; V = orth(Y) by CholeskyQR2 (the b x b Gram matrix reduced across the cluster in
+// rank order, Cholesky and the triangular inverse in float64 by one warp); Rayleigh-Ritz at the first iteration and every
+// kEigRR-th: T = V^T A V, cyclic Jacobi (float64, round-robin ordering, one CTA -- every CTA runs the same one, so all
+// agree without a broadcast), V <- V W.  It stops when every selected Ritz pair has ||A u - mu u|| <= 1e-5 max|mu|, or
+// at kEigMaxIter iterations, which sets the sticky non-converged flag.  The next step warm-starts from the stored Ritz
+// basis; the first starts from a fixed pseudo-random basis.  With D <= b, V spans everything and the first Rayleigh-Ritz
+// is the full Jacobi eigh of A.  Every reduction has a fixed order: two runs are bit-identical.
+enum { LRD_ENGAGED = 0, LRD_ITERS, LRD_RESID, LRD_NOCONV, LRD_ITERS_SUM, LRD_ITERS_MAX, LRD_SOLVES, LRD_WARM };
+constexpr int kLrdHdr = 16;
+constexpr int kLrdMaxDim = 512, kLrdMaxRank = 16;
+constexpr int kEigCtas = 8, kEigThreads = 512, kEigB = 48, kEigMaxIter = 300, kEigRR = 4, kJacobiSweeps = 30;
+constexpr float kEigTol = 1e-5f, kLamFloor = 1e-6f;
+
+static int lrd_basis_cols(int D, int k) { return std::min(D, 2 * k + 16); }
+
+// lrd_state: header | sigma[D] U[D,k] lam[k] (this step's metric) | n, mean[D] of the merged accumulator | mu, sd, -
+// [3D] of the final positions | Ritz basis [D, b] | merged covariance [D, D] | fold scratch | block accumulators
+struct LrdLayout {
+  size_t sigma, U, lam, cm, fin, basis, W, stats, cov, total;
+};
+static LrdLayout lrd_layout(int C, int D, int k) {
+  LrdLayout L{};
+  const size_t d = (size_t)D;
+  const int nb = cov_stat_blocks(C);
+  size_t o = kLrdHdr;
+  L.sigma = o; o += d;
+  L.U = o; o += d * k;
+  L.lam = o; o += k;
+  L.cm = o; o += 1 + d;
+  L.fin = o; o += 3 * d;
+  L.basis = o; o += d * lrd_basis_cols(D, k);
+  L.W = o; o += d * d;
+  L.stats = o; o += (size_t)nb * (2 + 2 * d);
+  L.cov = o; o += (size_t)nb * cov_block_floats(D);
+  L.total = o;
+  return L;
+}
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return v;
+}
+
+__device__ __forceinline__ float lrd_floor(float l) { return isnan(l) ? l : fmaxf(l, kLamFloor); }  // jnp.maximum keeps NaN
+
+// The gate and the diagonal fallback.  mu, sd [K, D]: mean and population std of each of K folds of n chains, pooled
+// here into the std of all K n chains.  Writes the engagement flag; the metric only when not engaged.
+__global__ void k_lrd_fallback(int D, int k, int K, int n, const float* __restrict__ mu, const float* __restrict__ sd,
+                               int gate, const float* __restrict__ cm, float* __restrict__ hdr, float* __restrict__ sigma,
+                               float* __restrict__ U, float* __restrict__ lam) {
+  const bool engaged = gate && cm[0] >= 2.f * (float)D;
+  if (threadIdx.x == 0) hdr[LRD_ENGAGED] = engaged ? 1.f : 0.f;
+  if (engaged) return;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    float m = 0.f;
+    for (int f = 0; f < K; ++f) m += mu[(size_t)f * D + d];
+    m /= (float)K;
+    float v = 0.f;
+    for (int f = 0; f < K; ++f) {
+      const float s = sd[(size_t)f * D + d], e = mu[(size_t)f * D + d] - m;
+      v += s * s + e * e;
+    }
+    const float s = K == 1 ? sd[d] : sqrtf(v / (float)K);
+    sigma[d] = s <= 0.f ? 1.f : s;
+    for (int j = 0; j < k; ++j) U[(size_t)d * k + j] = d == j ? 1.f : 0.f;
+  }
+  for (int j = threadIdx.x; j < k; j += blockDim.x) lam[j] = 1.f;
+}
+
+// the metric into the handle's low-rank block, in k_low_rank_prepare's layout
+__global__ void k_lrd_install(int D, int k, const float* __restrict__ sigma, const float* __restrict__ U,
+                              const float* __restrict__ lam, float* __restrict__ blk) {
+  float* sg = blk + (size_t)D * k;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < D * k; i += gridDim.x * blockDim.x) blk[i] = U[i];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < D) {
+    sg[i] = sigma[i];
+    sg[D + i] = 1.0f / sigma[i];
+  }
+  if (i < k) {
+    sg[2 * D + i] = lam[i] - 1.0f;
+    sg[2 * D + k + i] = 1.0f / sqrtf(lam[i]) - 1.0f;
+  }
+}
+
+// damping input (:599-634, _low_rank_precondition_pos :215-239): P = (x + ((x U)(lam^-1/2 - 1)) U^T) / sigma with x the
+// chain's position minus its fold's mean (the transform is linear, so this is the fold-centred transformed position).
+// One warp per chain, the row in registers.
+__global__ void k_lrd_transform(int C, int n, int D, int k, const float* __restrict__ q, const float* __restrict__ mu,
+                                const float* __restrict__ sigma, const float* __restrict__ U, const float* __restrict__ lam,
+                                float* __restrict__ P) {
+  const int chain = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (chain >= C) return;
+  constexpr int NS = kLrdMaxDim / 32;
+  const float* m = mu + (size_t)(chain / n) * D;
+  float x[NS], y[NS];
+#pragma unroll
+  for (int s = 0; s < NS; ++s) {
+    const int d = s * 32 + lane;
+    x[s] = d < D ? q[(size_t)chain * D + d] - m[d] : 0.f;
+    y[s] = x[s];
+  }
+  for (int j = 0; j < k; ++j) {
+    float t = 0.f;
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+      const int d = s * 32 + lane;
+      if (d < D) t = fmaf(x[s], U[(size_t)d * k + j], t);
+    }
+    t = warp_sum(t) * (1.0f / sqrtf(lam[j]) - 1.0f);
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+      const int d = s * 32 + lane;
+      if (d < D) y[s] = fmaf(U[(size_t)d * k + j], t, y[s]);
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < NS; ++s) {
+    const int d = s * 32 + lane;
+    if (d < D) P[(size_t)chain * D + d] = y[s] / sigma[d];
+  }
+}
+
+__device__ __forceinline__ float eig_hash(uint32_t i, uint32_t j) {  // cold-start basis entry in [-1, 1)
+  uint32_t x = (i * 0x9E3779B1u) ^ ((j + 0x7F4A7C15u) * 0x85EBCA77u);
+  x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16;
+  return (float)(x >> 8) * (2.0f / 16777216.0f) - 1.0f;
+}
+
+static size_t eig_rows(int D) { return (size_t)(D + kEigCtas - 1) / kEigCtas; }
+__host__ __device__ inline size_t round4(size_t n) { return (n + 3) & ~(size_t)3; }
+static size_t eig_smem_bytes(int D) {
+  const size_t RW = eig_rows(D);
+  return (3 * kEigB * kEigB + 2 * kEigB) * sizeof(double) + (kEigB + 16) * sizeof(int) +
+         (round4(D) + round4(RW * (D + 1)) + 3 * RW * kEigB) * sizeof(float);
+}
+
+namespace cg = cooperative_groups;
+
+// the eigensolver (see above).  gate && n >= 2 D of the merged accumulator, else nothing.  cm: n, mean; W: merged
+// covariance [D, D].  Writes sigma, U (top k by |mu|, descending), lam (floored), the Ritz basis and the diagnostics.
+__global__ void __cluster_dims__(kEigCtas, 1, 1) __launch_bounds__(kEigThreads)
+    k_lrd_eig(int D, int k, int B, int gate, const float* __restrict__ cm, const float* __restrict__ W,
+              float* __restrict__ hdr, float* __restrict__ sigma, float* __restrict__ U, float* __restrict__ lam,
+              float* __restrict__ basis) {
+  if (!(gate && cm[0] >= 2.f * (float)D)) return;
+  extern __shared__ __align__(16) unsigned char eig_smem[];
+  constexpr int NB = kEigB, NT = kEigThreads;
+  cg::cluster_group cl = cg::this_cluster();
+  const int rank = (int)cl.block_rank(), tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int RW = (D + kEigCtas - 1) / kEigCtas, r0 = rank * RW, nr = max(0, min(RW, D - r0)), lda = D + 1;
+  double* Gp = reinterpret_cast<double*>(eig_smem);  // this CTA's partial of a cluster reduction (read remotely)
+  double* G = Gp + NB * NB;                          // the reduced matrix (Cholesky factor in place)
+  double* Wm = G + NB * NB;                          // Jacobi eigenvectors / triangular inverse
+  double* theta = Wm + NB * NB;
+  double* cs = theta + NB;                           // Jacobi rotations of one round: c[24] | s[24]
+  int* order = reinterpret_cast<int*>(cs + NB);
+  int* flag = order + NB;                            // [0] Jacobi converged, [1] eigenpairs converged
+  float* sig = reinterpret_cast<float*>(flag + 16);
+  float* A = sig + round4(D);
+  float* V = A + round4((size_t)RW * lda);
+  float* Y = V + RW * NB;
+  float* buf = Y + RW * NB;
+  const bool warm = hdr[LRD_WARM] != 0.f;
+
+  // correlation (metric_estimators.py:599-605) minus the identity, this CTA's rows
+  for (int d = tid; d < D; d += NT) {
+    const float s = sqrtf(fmaxf(W[(size_t)d * D + d], 0.f));
+    sig[d] = s <= 0.f ? 1.f : s;
+  }
+  __syncthreads();
+  for (int e = tid; e < nr * D; e += NT) {
+    const int i = e / D, j = e - i * D, gi = r0 + i;
+    const float r = W[(size_t)gi * D + j] * (1.f / sig[gi]) * (1.f / sig[j]);
+    A[i * lda + j] = gi == j ? r - 1.f : r;
+  }
+  for (int e = tid; e < RW * NB; e += NT) {
+    const int i = e / NB, j = e - i * NB;
+    Y[e] = (i < nr && j < B) ? (warm ? basis[(size_t)(r0 + i) * B + j] : eig_hash(r0 + i, j)) : 0.f;
+  }
+  __syncthreads();
+
+  // G[0, n) = sum over the cluster's CTAs (rank order) of Gp[0, n)
+  auto cluster_sum = [&](int n) {
+    cl.sync();
+    for (int e = tid; e < n; e += NT) {
+      double s = 0.0;
+      for (int r = 0; r < kEigCtas; ++r) s += cl.map_shared_rank(Gp, r)[e];
+      G[e] = s;
+    }
+    cl.sync();
+  };
+  // Gp[i, j] = sum over this CTA's rows of X[row, i] Z[row, j]
+  auto gram = [&](const float* X, const float* Z) {
+    for (int e = tid; e < NB * NB; e += NT) {
+      const int i = e / NB, j = e - i * NB;
+      double s = 0.0;
+      if (i < B && j < B)
+        for (int r = 0; r < nr; ++r) s = fma((double)X[r * NB + i], (double)Z[r * NB + j], s);
+      Gp[e] = s;
+    }
+  };
+  // dst = src M for the B x B matrix M (upper triangular when tri), this CTA's rows
+  auto apply = [&](const float* src, const double* M, bool tri, float* dst) {
+    for (int e = tid; e < RW * NB; e += NT) {
+      const int r = e / NB, j = e - r * NB;
+      double s = 0.0;
+      if (r < nr && j < B)
+        for (int i = 0; i <= (tri ? j : B - 1); ++i) s = fma((double)src[r * NB + i], M[i * NB + j], s);
+      dst[e] = (float)s;
+    }
+    __syncthreads();
+  };
+  // dst = src R^-1 with src^T src = R^T R over the cluster (one CholeskyQR pass); src and dst are distinct
+  auto orth = [&](const float* src, float* dst) {
+    gram(src, src);
+    cluster_sum(NB * NB);
+    if (warp == 0) {
+      double mx = 0.0;
+      for (int i = 0; i < B; ++i) mx = fmax(mx, G[i * NB + i]);
+      if (mx > 0.0) {
+        const double fl = 1e-15 * mx;  // keeps a (numerically) dependent column finite; the second pass restores it
+        for (int j = 0; j < B; ++j) {
+          double s0 = 0.0, s1 = 0.0;
+          const int i0 = lane, i1 = lane + 32;
+          if (i0 >= j && i0 < B) {
+            s0 = G[j * NB + i0];
+            for (int t = 0; t < j; ++t) s0 -= G[t * NB + j] * G[t * NB + i0];
+          }
+          if (i1 >= j && i1 < B) {
+            s1 = G[j * NB + i1];
+            for (int t = 0; t < j; ++t) s1 -= G[t * NB + j] * G[t * NB + i1];
+          }
+          const double piv = __shfl_sync(0xffffffffu, (j >> 5) ? s1 : s0, j & 31);
+          const double rjj = sqrt(fmax(piv, fl));
+          __syncwarp();
+          if (i0 >= j && i0 < B) G[j * NB + i0] = i0 == j ? rjj : s0 / rjj;
+          if (i1 >= j && i1 < B) G[j * NB + i1] = i1 == j ? rjj : s1 / rjj;
+          __syncwarp();
+        }
+        for (int c = lane; c < B; c += 32)  // column c of R^-1 by back substitution
+          for (int i = B - 1; i >= 0; --i) {
+            double x = i == c ? 1.0 : 0.0;
+            if (i < c)
+              for (int t = i + 1; t <= c; ++t) x -= G[i * NB + t] * Wm[t * NB + c];
+            Wm[i * NB + c] = i <= c ? x / G[i * NB + i] : 0.0;
+          }
+      } else {  // A V = 0 (or NaN): keep the basis
+        for (int e = lane; e < NB * NB; e += 32) Wm[e] = (e / NB == e % NB) ? 1.0 : 0.0;
+      }
+    }
+    __syncthreads();
+    apply(src, Wm, true, dst);
+  };
+  // Y = A V; V is gathered slice by slice from every CTA through distributed shared memory
+  auto matmul = [&]() {
+    cl.sync();
+    const int rp = tid >> 4, cq = tid & 15;  // rows 2 rp, 2 rp + 1; columns 3 cq .. 3 cq + 2
+    float acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    for (int s = 0; s < kEigCtas; ++s) {
+      const int ns = max(0, min(RW, D - s * RW));
+      if (ns == 0) break;
+      const float4* src = reinterpret_cast<const float4*>(cl.map_shared_rank(V, s));
+      float4* dst = reinterpret_cast<float4*>(buf);
+      for (int e = tid; e < ns * (NB / 4); e += NT) dst[e] = src[e];
+      __syncthreads();
+      // rows past this CTA's RW are not stored: their threads read row RW - 1 and discard the result
+      const float* a0 = A + min(2 * rp, RW - 1) * lda + s * RW;
+      const float* a1 = A + min(2 * rp + 1, RW - 1) * lda + s * RW;
+      const float* b = buf + 3 * cq;
+      for (int jj = 0; jj < ns; ++jj) {
+        const float x0 = a0[jj], x1 = a1[jj];
+        const float b0 = b[jj * NB], b1 = b[jj * NB + 1], b2 = b[jj * NB + 2];
+        acc[0][0] = fmaf(x0, b0, acc[0][0]); acc[0][1] = fmaf(x0, b1, acc[0][1]); acc[0][2] = fmaf(x0, b2, acc[0][2]);
+        acc[1][0] = fmaf(x1, b0, acc[1][0]); acc[1][1] = fmaf(x1, b1, acc[1][1]); acc[1][2] = fmaf(x1, b2, acc[1][2]);
+      }
+      __syncthreads();
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        if (2 * rp + r < RW) Y[(2 * rp + r) * NB + 3 * cq + c] = (2 * rp + r < nr) ? acc[r][c] : 0.f;
+    __syncthreads();
+  };
+  // cyclic Jacobi on the symmetric Gp (order n2 = B rounded up to even, padded with zeros): eigenvalues to theta,
+  // eigenvectors to Wm.  Round-robin pairing, n2 / 2 disjoint rotations per round.
+  auto jacobi = [&]() {
+    const int n2 = B + (B & 1), half = n2 / 2;
+    double* M = Gp;
+    for (int e = tid; e < NB * NB; e += NT) {
+      const int i = e / NB, j = e - i * NB;
+      Wm[e] = i == j ? 1.0 : 0.0;
+      if (i >= B || j >= B) M[e] = 0.0;
+    }
+    __syncthreads();
+    auto pair_of = [&](int m, int rd, int& p, int& q) {
+      if (m == 0) { p = rd % (n2 - 1); q = n2 - 1; }
+      else { p = (rd + m) % (n2 - 1); q = (rd - m + n2 - 1) % (n2 - 1); }
+    };
+    for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
+      for (int rd = 0; rd < n2 - 1; ++rd) {
+        if (tid < half) {
+          int p, q;
+          pair_of(tid, rd, p, q);
+          const double app = M[p * NB + p], aqq = M[q * NB + q], apq = M[p * NB + q];
+          double c = 1.0, s = 0.0;
+          if (apq != 0.0) {
+            const double tau = (aqq - app) / (2.0 * apq);
+            const double t = (tau >= 0.0 ? 1.0 : -1.0) / (fabs(tau) + sqrt(1.0 + tau * tau));
+            c = 1.0 / sqrt(1.0 + t * t);
+            s = t * c;
+          }
+          cs[tid] = c;
+          cs[24 + tid] = s;
+        }
+        __syncthreads();
+        for (int e = tid; e < half * n2; e += NT) {  // rows p, q <- J^T rows
+          const int m = e / n2, col = e - m * n2;
+          int p, q;
+          pair_of(m, rd, p, q);
+          const double c = cs[m], s = cs[24 + m], x = M[p * NB + col], y = M[q * NB + col];
+          M[p * NB + col] = c * x - s * y;
+          M[q * NB + col] = s * x + c * y;
+        }
+        __syncthreads();
+        for (int e = tid; e < half * n2; e += NT) {  // columns p, q <- columns J, also for the eigenvectors
+          const int m = e / n2, row = e - m * n2;
+          int p, q;
+          pair_of(m, rd, p, q);
+          const double c = cs[m], s = cs[24 + m];
+          double x = M[row * NB + p], y = M[row * NB + q];
+          M[row * NB + p] = c * x - s * y;
+          M[row * NB + q] = s * x + c * y;
+          x = Wm[row * NB + p]; y = Wm[row * NB + q];
+          Wm[row * NB + p] = c * x - s * y;
+          Wm[row * NB + q] = s * x + c * y;
+        }
+        __syncthreads();
+      }
+      if (warp == 0) {
+        double off = 0.0, tot = 0.0;
+        for (int e = lane; e < n2 * n2; e += 32) {
+          const int i = e / n2, j = e - i * n2;
+          const double v = M[i * NB + j] * M[i * NB + j];
+          tot += v;
+          if (i != j) off += v;
+        }
+        off = warp_sum_d(off);
+        tot = warp_sum_d(tot);
+        if (lane == 0) flag[0] = off <= 1e-28 * tot ? 1 : 0;
+      }
+      __syncthreads();
+      const bool done = flag[0];
+      __syncthreads();
+      if (done) break;
+    }
+    for (int j = tid; j < B; j += NT) theta[j] = M[j * NB + j];
+    __syncthreads();
+  };
+
+  orth(Y, V);
+  orth(V, Y);
+  { float* t = V; V = Y; Y = t; }
+  int it = 0;
+  bool converged = false;
+  double resid = 0.0;
+  while (true) {
+    ++it;
+    matmul();
+    if (it == 1 || it % kEigRR == 0 || it == kEigMaxIter) {  // Rayleigh-Ritz and the residuals of the selected pairs
+      gram(V, Y);
+      cluster_sum(NB * NB);
+      for (int e = tid; e < NB * NB; e += NT) {
+        const int i = e / NB, j = e - i * NB;
+        Gp[e] = 0.5 * (G[i * NB + j] + G[j * NB + i]);
+      }
+      __syncthreads();
+      jacobi();
+      apply(V, Wm, false, buf);
+      for (int e = tid; e < RW * NB; e += NT) V[e] = buf[e];
+      __syncthreads();
+      apply(Y, Wm, false, buf);
+      for (int e = tid; e < RW * NB; e += NT) Y[e] = buf[e];
+      if (tid == 0) {  // scores |lam - 1| of the float32 eigenvalues it returns, descending; ties: the larger lam first
+        for (int j = 0; j < B; ++j) order[j] = j;  // (argsort(scores)[::-1] over eigh's ascending eigenvalues)
+        auto lam_f = [&](int j) { return (float)theta[j] + 1.0f; };
+        for (int m = 0; m < B; ++m) {
+          int best = m;
+          for (int j = m + 1; j < B; ++j) {
+            const float lj = lam_f(order[j]), lb = lam_f(order[best]);
+            const float a = fabsf(lj - 1.0f), b = fabsf(lb - 1.0f);
+            if (a > b || (a == b && lj > lb)) best = j;
+          }
+          const int t = order[m]; order[m] = order[best]; order[best] = t;
+        }
+      }
+      __syncthreads();
+      if (warp < k) {
+        const int j = order[warp];
+        const double th = theta[j];
+        double s = 0.0;
+        for (int r = lane; r < nr; r += 32) {
+          const double v = (double)Y[r * NB + j] - th * (double)V[r * NB + j];
+          s = fma(v, v, s);
+        }
+        s = warp_sum_d(s);
+        if (lane == 0) Gp[warp] = s;
+      }
+      cluster_sum(k);
+      if (tid == 0) {
+        const double mx = fabs(theta[order[0]]);
+        double rmax = 0.0;
+        for (int m = 0; m < k; ++m) rmax = fmax(rmax, sqrt(G[m]));
+        flag[1] = rmax <= (double)kEigTol * mx ? 1 : 0;
+        cs[0] = mx > 0.0 ? rmax / mx : rmax;  // cs is free between Jacobi calls: it hands the residual to every thread
+      }
+      __syncthreads();
+      converged = flag[1] != 0;
+      resid = cs[0];
+      __syncthreads();
+      if (converged || it == kEigMaxIter) break;
+    }
+    orth(Y, V);
+    orth(V, Y);
+    { float* t = V; V = Y; Y = t; }
+  }
+  for (int e = tid; e < nr * k; e += NT) {
+    const int i = e / k, m = e - i * k;
+    U[(size_t)(r0 + i) * k + m] = V[i * NB + order[m]];
+  }
+  for (int e = tid; e < nr * B; e += NT) {
+    const int i = e / B, j = e - i * B;
+    basis[(size_t)(r0 + i) * B + j] = V[i * NB + j];
+  }
+  if (rank == 0) {
+    for (int d = tid; d < D; d += NT) sigma[d] = sig[d];
+    for (int m = tid; m < k; m += NT) lam[m] = lrd_floor((float)theta[order[m]] + 1.0f);
+    if (tid == 0) {
+      hdr[LRD_ITERS] = (float)it;
+      hdr[LRD_RESID] = (float)resid;
+      if (!converged) hdr[LRD_NOCONV] = 1.f;
+      hdr[LRD_ITERS_SUM] += (float)it;
+      hdr[LRD_ITERS_MAX] = fmaxf(hdr[LRD_ITERS_MAX], (float)it);
+      hdr[LRD_SOLVES] += 1.f;
+      hdr[LRD_WARM] = 1.f;
+    }
+  }
+  cl.sync();  // no CTA leaves while another may still read its shared memory
+}
 static long long next_pow2(long long n) {
   long long p = 1;
   while (p < n) p <<= 1;
@@ -382,5 +847,128 @@ extern "C" int bjx_gather_rows(bjx_handle_t h, const int32_t* perm, const float*
   if (rows == 0) return 0;
   k_gather_rows<<<(unsigned)((rows + 3) / 4), 128, 0, h->stream>>>(perm, src, dst, (int)rows, width);
   BJX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- MEADS-LRD entry points -----------------------------------------------------------------------------------------
+extern "C" size_t bjx_meads_lrd_state_floats(int32_t n_chains, int32_t dim, int32_t rank) {
+  if (n_chains < 1 || dim < 1 || dim > kLrdMaxDim || rank < 1 || rank > kLrdMaxRank || rank > dim) return 0;
+  return lrd_layout(n_chains, dim, rank).total;
+}
+extern "C" size_t bjx_meads_lrd_scratch_floats(int32_t n_chains, int32_t dim, int32_t num_folds) {
+  return bjx_meads_scratch_floats(n_chains, dim, num_folds) + (size_t)2 * num_folds * dim + (size_t)n_chains +
+         (size_t)n_chains * dim;
+}
+
+// the handle's rank-k low-rank metric (installed once by the caller; the warm-up rewrites it in place)
+static int lrd_check(bjx_handle_t h, int& k) {
+  const int D = h->cfg.dim;
+  if (h->metric_kind != BJX_METRIC_LOW_RANK || !h->lr_block || h->lr_k < 1)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "MEADS-LRD needs a low-rank metric on the handle (bjx_set_metric_low_rank)");
+  k = h->lr_k;
+  if (D > kLrdMaxDim || k > kLrdMaxRank || k > D)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, "MEADS-LRD is built for dim <= 512 and 1 <= rank <= min(16, dim)");
+  return 0;
+}
+
+static int lrd_eigensolve(bjx_handle_t h, int k, int gate, const LrdLayout& L, float* ls) {
+  const int D = h->cfg.dim;
+  const size_t smem = eig_smem_bytes(D);
+  {  // the shared-memory opt-in, once per device, at the size of the largest dimension
+    static std::mutex mu;
+    static bool done[64] = {};
+    std::lock_guard<std::mutex> lock(mu);
+    const int dev = h->cfg.device;
+    if (dev < 0 || dev >= 64 || !done[dev]) {
+      BJX_CUDA(cudaFuncSetAttribute(k_lrd_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eig_smem_bytes(kLrdMaxDim)));
+      if (dev >= 0 && dev < 64) done[dev] = true;
+    }
+  }
+  k_lrd_eig<<<kEigCtas, kEigThreads, smem, h->stream>>>(D, k, lrd_basis_cols(D, k), gate, ls + L.cm, ls + L.W, ls,
+                                                       ls + L.sigma, ls + L.U, ls + L.lam, ls + L.basis);
+  BJX_CHECK_LAUNCH("k_lrd_eig");
+  return 0;
+}
+
+extern "C" int bjx_meads_lrd_update(bjx_handle_t h, const float* q, const float* grad, int32_t num_folds, int32_t t,
+                                    int32_t in_window, float step_size_multiplier, float damping_slowdown, float* state,
+                                    float* lrd_state, float* scratch) {
+  if (!h || !q || !grad || !state || !lrd_state || !scratch) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  const int C = h->cfg.n_chains, D = h->cfg.dim, K = num_folds;
+  if (K < 1 || K > 64) return bjx_fail(h, BJX_E_INVALID, "num_folds must be in [1, 64]");
+  if (C % K != 0) return bjx_fail(h, BJX_E_INVALID, "num_chains must be divisible by num_folds");
+  const int n = C / K;
+  if (n < 2) return bjx_fail(h, BJX_E_INVALID, "MEADS needs at least 2 chains per fold");
+  int k = 0;
+  int rc = lrd_check(h, k);
+  if (rc) return rc;
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const LrdLayout L = lrd_layout(C, D, k);
+  float* ls = lrd_state;
+  float* mu = scratch;
+  float* sd = mu + (size_t)K * D;
+  float* mus = sd + (size_t)K * D;
+  float* rg = mus + (size_t)K * D;
+  float* rq = rg + C;
+  float* tiles = rq + C;
+  const int T = (D + 31) / 32, pairs = meads_pairs(D);
+  float* ones = tiles + (size_t)2 * K * pairs;
+  float* zeros = ones + (size_t)K * D;
+  float* rdummy = zeros + (size_t)K * D;
+  float* P = rdummy + C;
+  cudaStream_t s = h->stream;
+  // the fold statistics of bjx_meads_update: the step sizes come from these unchanged.  Only the gradient half of the
+  // Gram tiles (grid y = 1) is formed here; the position half comes from the transformed positions below.
+  k_meads_moments<<<dim3(T, K), dim3(32, 8), 0, s>>>(n, D, q, mu, sd, mus);
+  k_meads_rows<<<(C + 3) / 4, 128, 0, s>>>(C, n, D, q, grad, sd, mus, rg, rq);
+  k_meads_gram<<<dim3(pairs, 1, K), dim3(32, 32), 0, s>>>(n, D, T, q, grad, sd, mus, tiles);
+  BJX_CHECK_LAUNCH("k_meads_gram");
+  // this step's metric (:549-568)
+  if (in_window) {
+    launch_cov_fold(C, D, q, ls + L.stats, ls + L.cov, s);
+    launch_cov_merge(C, D, ls + L.cov, ls + L.W, ls + L.cm, s);
+    BJX_CHECK_LAUNCH("launch_cov_merge");
+  }
+  k_lrd_fallback<<<1, 512, 0, s>>>(D, k, K, n, mu, sd, in_window ? 1 : 0, ls + L.cm, ls, ls + L.sigma, ls + L.U, ls + L.lam);
+  BJX_CHECK_LAUNCH("k_lrd_fallback");
+  if (in_window) {
+    rc = lrd_eigensolve(h, k, 1, L, ls);
+    if (rc) return rc;
+  }
+  k_lrd_install<<<(D + 255) / 256, 256, 0, s>>>(D, k, ls + L.sigma, ls + L.U, ls + L.lam, h->lr_block);
+  // damping from the fold-centred, low-rank-preconditioned positions (:599-634): their statistics replace the position
+  // half of the fold statistics (rows of X X^T, and the tiles at offset `pairs`) with unit scales and zero means
+  k_lrd_transform<<<(C + 7) / 8, 256, 0, s>>>(C, n, D, k, q, mu, ls + L.sigma, ls + L.U, ls + L.lam, P);
+  k_fill2<<<(K * D + 255) / 256, 256, 0, s>>>(ones, K * D, 1.0f, zeros, 0.0f);
+  k_meads_rows<<<(C + 3) / 4, 128, 0, s>>>(C, n, D, P, P, ones, zeros, rdummy, rq);
+  k_meads_gram<<<dim3(pairs, 1, K), dim3(32, 32), 0, s>>>(n, D, T, P, P, ones, zeros, tiles + pairs);
+  k_meads_finish<<<1, 256, 0, s>>>(n, D, K, pairs, t, step_size_multiplier, damping_slowdown, sd, rg, rq, tiles, state);
+  BJX_CHECK_LAUNCH("k_meads_finish");
+  return 0;
+}
+
+extern "C" int bjx_meads_lrd_metric(bjx_handle_t h, float* lrd_state, const float* final_q, float* sigma_out, float* U_out,
+                                    float* lam_out) {
+  if (!h || !lrd_state || !final_q || !sigma_out || !U_out || !lam_out) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  int k = 0;
+  int rc = lrd_check(h, k);
+  if (rc) return rc;
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  if (C < 2) return bjx_fail(h, BJX_E_INVALID, "MEADS-LRD needs at least 2 chains");
+  const LrdLayout L = lrd_layout(C, D, k);
+  float* ls = lrd_state;
+  float* fin = ls + L.fin;
+  cudaStream_t s = h->stream;
+  // the last accumulator if it holds 2 D samples, else the fallback on the final positions (:746-771)
+  k_meads_moments<<<dim3((D + 31) / 32, 1), dim3(32, 8), 0, s>>>(C, D, final_q, fin, fin + D, fin + 2 * D);
+  launch_cov_merge(C, D, ls + L.cov, ls + L.W, ls + L.cm, s);
+  k_lrd_fallback<<<1, 512, 0, s>>>(D, k, 1, C, fin, fin + D, 1, ls + L.cm, ls, ls + L.sigma, ls + L.U, ls + L.lam);
+  BJX_CHECK_LAUNCH("k_lrd_fallback");
+  rc = lrd_eigensolve(h, k, 1, L, ls);
+  if (rc) return rc;
+  BJX_CUDA(cudaMemcpyAsync(sigma_out, ls + L.sigma, (size_t)D * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  BJX_CUDA(cudaMemcpyAsync(U_out, ls + L.U, (size_t)D * k * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  BJX_CUDA(cudaMemcpyAsync(lam_out, ls + L.lam, (size_t)k * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return 0;
 }

@@ -203,6 +203,32 @@ size_t bjx_meads_state_floats(int32_t num_folds, int32_t dim);
 size_t bjx_meads_scratch_floats(int32_t n_chains, int32_t dim, int32_t num_folds);
 int bjx_meads_update(bjx_handle_t h, const float* q, const float* grad, int32_t num_folds, int32_t t,
                      float step_size_multiplier, float damping_slowdown, float* state, float* scratch);
+/* MEADS-LRD (meads_adaptation.py:459-784 with low_rank_rank = k): ONE low-rank metric for all chains per warm-up step.
+ * The handle must hold a rank-k low-rank metric (bjx_set_metric_low_rank, installed once with the fallback values);
+ * bjx_meads_lrd_update rewrites that metric's block in place on the stream (no allocation, no host round trip).
+ * Built for dim <= 512, 1 <= k <= min(16, dim), one GPU; otherwise BJX_E_UNSUPPORTED.
+ * lrd_state float32 [bjx_meads_lrd_state_floats], zero-filled before the first step; its first 16 floats are
+ *   [0] 1 if this step's metric came from the accumulator   [1] eigensolver iterations of the last solve
+ *   [2] its largest residual ||A u - mu u|| / max|mu|       [3] 1 once any solve stopped at the iteration cap (sticky)
+ *   [4] sum and [5] maximum of the iterations over solves   [6] number of solves   [7] 1 once a Ritz basis is stored
+ * followed by sigma[D] | U[D,k] | lam[k], the metric of the last step.  scratch: bjx_meads_lrd_scratch_floats.
+ * k is read from the handle's low-rank metric on every call: an lrd_state sized for (C, D, k) must only be used
+ * with a handle of C chains and D dims holding a rank-k metric (a different rank would address the state wrongly).
+ * bjx_meads_lrd_update: with in_window, folds q [C,D] into the windowed covariance accumulator (cgl_update_batch);
+ * the metric is the top-k pairs by |lam - 1| of the accumulated correlation matrix when in_window and it holds
+ * >= 2 dim samples, else the fallback (std of q over all chains, pooled from the per-fold mean and std, so equal
+ * to a direct std up to float32 rounding; eye(dim, k), ones(k)); lam floored at 1e-6.  state
+ * as in bjx_meads_update: the step sizes are those of bjx_meads_update, alpha / delta come from the fold-centred
+ * positions under the low-rank transform (x + ((x U)(lam^-1/2 - 1)) U^T) / sigma (:599-634).  Run bjx_ghmc_step with
+ * the state's step_size / alpha / delta rows and imm_rows = msqrt_rows = NULL.
+ * bjx_meads_lrd_metric: the final metric (:746-771) -- the accumulator if it holds >= 2 dim samples, else the
+ * fallback on final_q -- into sigma_out [D], U_out [D,k], lam_out [k] (device). */
+size_t bjx_meads_lrd_state_floats(int32_t n_chains, int32_t dim, int32_t rank);
+size_t bjx_meads_lrd_scratch_floats(int32_t n_chains, int32_t dim, int32_t num_folds);
+int bjx_meads_lrd_update(bjx_handle_t h, const float* q, const float* grad, int32_t num_folds, int32_t t, int32_t in_window,
+                         float step_size_multiplier, float damping_slowdown, float* state, float* lrd_state, float* scratch);
+int bjx_meads_lrd_metric(bjx_handle_t h, float* lrd_state, const float* final_q, float* sigma_out, float* U_out,
+                         float* lam_out);
 /* maximum_eigenvalue (meads_adaptation.py:787-817) of one float32 [n, d] device matrix; out: ONE device float */
 size_t bjx_maximum_eigenvalue_scratch_floats(int64_t n, int32_t d);
 int bjx_maximum_eigenvalue(bjx_handle_t h, const float* x, int64_t n, int32_t d, float* out, float* scratch);
