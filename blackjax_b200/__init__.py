@@ -18,7 +18,8 @@ from .mcmc import hmc as _hmc
 from .mcmc import nuts as _nuts
 from .mcmc import dynamic_hmc as _dynamic_hmc
 from .mcmc import ghmc as _ghmc
-from .util import run_inference_algorithm, sample_hmc_native, sample_nuts_native  # noqa: F401
+from .mcmc import mclmc as _mclmc
+from .util import run_inference_algorithm, sample_hmc_native, sample_mclmc_native, sample_nuts_native  # noqa: F401
 
 hmc = GenerateSamplingAPI(_hmc.as_top_level_api, _hmc.init, _hmc.build_kernel)     # blackjax/__init__.py:111
 nuts = GenerateSamplingAPI(_nuts.as_top_level_api, _nuts.init, _nuts.build_kernel)  # blackjax/__init__.py:112
@@ -37,5 +38,6 @@ dmhmc = GenerateSamplingAPI(                                                    
 )
 
 ghmc = GenerateSamplingAPI(_ghmc.as_top_level_api, _ghmc.init, _ghmc.build_kernel)   # blackjax/__init__.py:139
+mclmc = GenerateSamplingAPI(_mclmc.as_top_level_api, _mclmc.init, _mclmc.build_kernel)  # blackjax/__init__.py:141
 
 __version__ = "0.1.0"

@@ -77,10 +77,11 @@ class Engine:
             pass
 
     # -- metric ---------------------------------------------------------------------------------
-    def set_metric(self, inverse_mass_matrix):
+    def set_metric(self, inverse_mass_matrix, diagonal_only=False):
         """1-D => diagonal, 2-D [D,D] => dense, 2-D [C,D] => per-chain diagonal, 3-D [C,D,D] => per-chain dense
         (blackjax/mcmc/metrics.py:701-729 semantics incl. the ValueError; the per-chain layouts are what jax.vmap
-        over chains gives the reference)."""
+        over chains gives the reference).  ``diagonal_only`` (MCLMC, whose metric is always diagonal): a 2-D array is
+        per-chain diagonal [C,D] whatever C and D are."""
         imm = inverse_mass_matrix
         from .mcmc.metrics import LowRankMetric
         if isinstance(imm, LowRankMetric):  # metrics.gaussian_euclidean_low_rank (metrics.py:349-467)
@@ -97,6 +98,11 @@ class Engine:
             if imm.shape[0] != self.D:
                 raise ValueError(f"inverse_mass_matrix has {imm.shape[0]} entries, expected {self.D}")
             kind = _lib.METRIC_DIAG
+        elif diagonal_only and imm.ndim == 2:
+            if tuple(imm.shape) != (self.C, self.D):
+                raise ValueError(f"per-chain diagonal inverse_mass_matrix has shape {tuple(imm.shape)}, "
+                                 f"expected ({self.C}, {self.D})")
+            kind = _lib.METRIC_DIAG_PER_CHAIN
         elif imm.ndim == 2 and tuple(imm.shape) == (self.D, self.D):
             kind = _lib.METRIC_DENSE
         elif imm.ndim == 2 and tuple(imm.shape) == (self.C, self.D):
@@ -111,7 +117,7 @@ class Engine:
         check(lib().bjx_set_metric(self.h, kind, ptr(imm)), self.h)
         return imm
 
-    def ensure_metric(self, inverse_mass_matrix):
+    def ensure_metric(self, inverse_mass_matrix, diagonal_only=False):
         """Install the metric unless this exact tensor CONTENT is already installed: the cache key is (storage pointer,
         shape, torch's in-place version counter), so an in-place update of the caller's tensor re-derives
         mass_matrix_sqrt and the dense operand planes instead of silently keeping stale ones."""
@@ -120,10 +126,10 @@ class Engine:
         if isinstance(imm, LowRankMetric):
             key = tuple((t.data_ptr(), tuple(t.shape), t._version, str(t.device)) for t in imm)
         else:
-            key = ((imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device)) if isinstance(imm, torch.Tensor)
-                   else None)
+            key = ((imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device), diagonal_only)
+                   if isinstance(imm, torch.Tensor) else None)
         if key is None or key != self._imm_key:
-            installed = self.set_metric(imm)
+            installed = self.set_metric(imm, diagonal_only)
             # a converted copy (dtype / device / layout) is owned by the engine: key on the caller's tensor all the same
             self._imm_key = key
             return installed
@@ -188,13 +194,14 @@ class Engine:
                                    ptr(_f32(ps, (self.C, self.D))), ptr(out)), self.h)
         return out.bool()
 
-    def _eps(self, step_size):
+    def _eps(self, step_size, name="step_size"):
+        """A per-chain parameter (step size, MCLMC's L): scalar -> (value, None); [C] tensor -> (0, device array)."""
         if isinstance(step_size, torch.Tensor) and step_size.ndim >= 1:
-            return 0.0, _f32(step_size.to(self.device), (self.C,), "step_size")
+            return 0.0, _f32(step_size.to(self.device), (self.C,), name)
         return float(step_size), None
 
-    def _info(self, fields):
-        info = _lib.Info()
+    def _info(self, fields, struct=_lib.Info):
+        info = struct()
         for k, v in fields.items():
             setattr(info, k, ptr(v))
         return info
@@ -250,6 +257,29 @@ class Engine:
         if key_integrator is not None:
             self._keymode = None  # per-call override: re-establish the key mode on the next ordinary call
         return qo, lo, go
+
+    def mclmc_init(self, keys, q, chain_offset=0):
+        """mclmc.init: (logp, grad, unit momentum)."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        logp = torch.empty(self.C, dtype=torch.float32, device=self.device)
+        g, p = torch.empty_like(q), torch.empty_like(q)
+        check(lib().bjx_mclmc_init(self.h, ptr(keys), ptr(q), ptr(logp), ptr(g), ptr(p)), self.h)
+        return logp, g, p
+
+    def mclmc_step_(self, keys, q, p, logp, g, step_size, L, energy_cutoff, info_fields=None, chain_offset=0):
+        """One MCLMC transition IN PLACE on (q, p, logp, g)."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        eps, eps_dev = self._eps(step_size)
+        L, L_dev = self._eps(L, "L")
+        info = self._info(info_fields or {}, _lib.MclmcInfo)
+        check(lib().bjx_mclmc_step(self.h, ptr(keys), ptr(_f32(q, (self.C, self.D), "position")),
+                                   ptr(_f32(p, (self.C, self.D), "momentum")), ptr(_f32(logp, (self.C,), "logdensity")),
+                                   ptr(_f32(g, (self.C, self.D), "logdensity_grad")), eps, ptr(eps_dev), L, ptr(L_dev),
+                                   float(energy_cutoff), C.byref(info)), self.h)
+        self._mclmc_keepalive = (eps_dev, L_dev)  # the launch is asynchronous
 
     def nuts_last_stats(self):
         a, b = C.c_int64(), C.c_int64()

@@ -33,6 +33,10 @@ class Info(C.Structure):
         "left_momentum", "right_position", "right_momentum")]
 
 
+class MclmcInfo(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("kinetic_change", "energy_change", "nonans")]
+
+
 class BjxError(RuntimeError):
     pass
 
@@ -67,6 +71,11 @@ _SIGNATURES = {
                                 C.c_int32, C.POINTER(Info)]),
     "bjx_hmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, C.c_int32, C.c_int32,
                                  _f32p, C.c_int32, _f32p]),
+    "bjx_mclmc_init": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p]),
+    "bjx_mclmc_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, _f32p,
+                                 C.c_float, C.POINTER(MclmcInfo)]),
+    "bjx_mclmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, _f32p,
+                                   C.c_float, C.c_int32, _f32p, C.c_int32, _f32p]),
     "bjx_nuts_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
                                 C.c_int32, C.POINTER(Info), _f32p, _f32p]),
     "bjx_nuts_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, C.c_int32, _f32p,

@@ -51,10 +51,7 @@ int bjx_big_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
                      float* q_out, float* logp_out, float* g_out, float eps, const float* eps_dev, int L,
                      const bjx::InfoPtrs& info);
 
-// Execution path of a call.  ROUTE_ROWS: the warp-per-chain row kernels (dim <= 1024, bjx_launch.cuh); ROUTE_BIG: the
-// CTA-per-chain kernels (1024 < dim, bjx_big.cu); ROUTE_DENSE: the tensor-core dense path (bjx_dense.cu), taken by a dense
-// Gaussian target or a dense metric beyond 128 dims.
-enum Route { ROUTE_ROWS, ROUTE_BIG, ROUTE_DENSE };
+// Execution path of a call (enum Route: bjx_internal.h).
 static Route rows_or_big(bjx_handle_t h) { return h->sc == SC_BIG ? ROUTE_BIG : ROUTE_ROWS; }
 // where the target alone is evaluated (bjx_init_state)
 static Route target_route(bjx_handle_t h) {
@@ -67,7 +64,7 @@ static Route metric_route(bjx_handle_t h) {
   return rows_or_big(h);
 }
 // where a transition, which needs both, runs
-static Route transition_route(bjx_handle_t h) {
+Route transition_route(bjx_handle_t h) {
   if (target_route(h) == ROUTE_DENSE || metric_route(h) == ROUTE_DENSE) return ROUTE_DENSE;
   return rows_or_big(h);
 }
@@ -343,7 +340,7 @@ extern "C" int bjx_get_mass_matrix_sqrt(bjx_handle_t h, const float** out) {
   return 0;
 }
 
-static Params make_params(bjx_handle_t h, float eps, const float* eps_dev) {
+Params make_params(bjx_handle_t h, float eps, const float* eps_dev) {
   Params P;
   P.C = h->cfg.n_chains;
   P.D = h->cfg.dim;
@@ -380,7 +377,7 @@ static Params make_params(bjx_handle_t h, float eps, const float* eps_dev) {
   return P;
 }
 
-static int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, LaunchArgs& a) {
+int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, LaunchArgs& a) {
   a.stream = h->stream;
   a.general_integrator = h->general_integrator;
   const bool dm = h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK;
@@ -403,7 +400,7 @@ static int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, Launch
   return 0;
 }
 
-static int check_ready(bjx_handle_t h, bool need_metric, const void* const* ptrs, int n) {
+int check_ready(bjx_handle_t h, bool need_metric, const void* const* ptrs, int n) {
   if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
   if (need_metric && h->metric_kind < 0) return bjx_fail(h, BJX_E_STATE, "metric not set: call bjx_set_metric first");
   for (int i = 0; i < n; ++i) {
@@ -645,7 +642,7 @@ extern "C" int bjx_mhmc_step(bjx_handle_t h, const uint32_t* keys, const float* 
 
 // ---- run loops ------------------------------------------------------------------------------------------
 // Step keys of a run loop: split(rng_key, num_steps) into h->sample_keys, on the device (util.py:203).
-static int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps) {
+int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps) {
   int rc = bjx_grow(h, h->sample_keys, h->sample_keys_cap, (size_t)num_steps, 2 * sizeof(uint32_t));
   if (rc) return rc;
   launch_prng_split(rng_key, 1, num_steps, h->sample_keys, h->stream);
@@ -653,16 +650,8 @@ static int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_step
   return 0;
 }
 
-// For its lifetime every chain's key derives from one step key (bjx_set_key_mode 1); the caller's mode comes back after.
-struct SharedStepKeys {
-  bjx_handle_t h;
-  int saved;
-  explicit SharedStepKeys(bjx_handle_t h_) : h(h_), saved(h_->key_shared) { h->key_shared = 1; }
-  ~SharedStepKeys() { h->key_shared = saved; }
-};
-
 // history (optional) receives the positions after every `thin`-th transition: row (t + 1) / thin - 1 after transition t
-static int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q) {
+int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q) {
   if (!history || ((t + 1) % thin) != 0) return 0;
   const size_t row = (size_t)h->cfg.n_chains * h->cfg.dim;
   BJX_CUDA(cudaMemcpyAsync(history + (size_t)((t + 1) / thin - 1) * row, q, row * sizeof(float), cudaMemcpyDeviceToDevice,

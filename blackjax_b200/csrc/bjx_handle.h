@@ -79,6 +79,14 @@ int bjx_grow(bjx_handle_t h, T*& buf, size_t& cap, size_t need, size_t unit_byte
   return 0;
 }
 
+// For its lifetime every chain's key derives from one step key (bjx_set_key_mode 1); the caller's mode comes back after.
+struct SharedStepKeys {
+  bjx_handle_t h;
+  int saved;
+  explicit SharedStepKeys(bjx_handle_t h_) : h(h_), saved(h_->key_shared) { h->key_shared = 1; }
+  ~SharedStepKeys() { h->key_shared = saved; }
+};
+
 // Error idiom of every entry point: a failing CUDA call or kernel launch returns its cudaError_t, message in h->err.
 #define BJX_CUDA(call)                                            \
   do {                                                            \

@@ -37,3 +37,25 @@ size_t cov_block_floats(int D);
 void launch_cov_fold(int C, int D, const float* q, float* stats, float* cov, cudaStream_t s);
 void launch_cov_merge(int C, int D, const float* cov, float* out, float* count_mean, cudaStream_t s);
 }  // namespace bjx
+
+// Host-side routing and run-loop helpers of bjx_api.cu, shared with the entry points of other translation units.
+typedef struct bjx_handle_s* bjx_handle_t;
+namespace bjx {
+struct Params;
+struct LaunchArgs;
+}  // namespace bjx
+// Execution path of a call.  ROUTE_ROWS: the warp-per-chain row kernels (dim <= 1024, bjx_launch.cuh); ROUTE_BIG: the
+// CTA-per-chain kernels (1024 < dim, bjx_big.cu); ROUTE_DENSE: the tensor-core dense path (bjx_dense.cu), taken by a dense
+// Gaussian target or a dense metric beyond 128 dims.
+enum Route { ROUTE_ROWS, ROUTE_BIG, ROUTE_DENSE };
+Route transition_route(bjx_handle_t h);                  // where a transition, which needs target and metric, runs
+bjx::Params make_params(bjx_handle_t h, float eps, const float* eps_dev);
+// launches kernel_id of the handle's (target, size class, metric, integrator) variant; target_dependent = false takes the
+// target-independent instance
+int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, bjx::LaunchArgs& a);
+// null handle / metric not set / null or misaligned state arrays; selects the handle's device
+int check_ready(bjx_handle_t h, bool need_metric, const void* const* ptrs, int n);
+// split(rng_key, num_steps) into h->sample_keys (util.py:203)
+int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps);
+// history row (t + 1) / thin - 1 = q after transition t, when (t + 1) % thin == 0
+int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q);

@@ -10,7 +10,8 @@
 namespace bjx {
 
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
-enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS };
+enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
+               K_MCLMC };
 
 struct LaunchArgs {
   Params P;
@@ -18,6 +19,7 @@ struct LaunchArgs {
   InfoPtrs info;
   GhmcArgs ghmc;
   NutsSampleArgs sample;
+  MclmcArgs mclmc;
   int grid_override;    // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
@@ -98,6 +100,13 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
     case K_GHMC:
       k_ghmc_transition<R, TK, DM, GEN><<<grid, block, smem, st>>>(a.P, a.keys, a.q_out, a.logp_out, a.g_out, a.ghmc, a.info);
       return 0;
+    case K_MCLMC:  // diagonal metrics only: the host rejects the others before dispatch
+      if constexpr (!DM) {
+        k_mclmc_transition<R, TK, DM, GEN><<<grid, block, smem, st>>>(a.P, a.keys, a.q_out, a.p_io, a.logp_out, a.g_out,
+                                                                       a.mclmc);
+        return 0;
+      }
+      break;
     case K_NUTS_CHAINS: {
       size_t sm_bytes = smem + (a.sample.ckpt_smem ? sizeof(float) * kWarpsPerBlock * 2 * a.sample.max_doublings * a.P.D : 0);
       // persistent grid: every CTA that fits (registers, checkpoint shared memory) on each of the grid_override SMs

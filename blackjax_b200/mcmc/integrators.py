@@ -18,13 +18,22 @@ _b1o, _a1o, _b2o, _a2o = 0.08398315262876693, 0.2539785108410595, 0.682236533571
 _b3o, _a3o = 0.5 - _b1o - _b2o, 1.0 - 2.0 * (_a1o + _a2o)
 omelyan = (_b1o, _a1o, _b2o, _a2o, _b3o, _a3o, _b3o, _a2o, _b2o, _a1o, _b1o)        # integrators.py:363-369
 
+# The isokinetic integrators of MCLMC (integrators.py:533-539) run the same tables: mclmc's kernel interprets even entries as
+# the ESH momentum update and odd entries as the position update.
+isokinetic_velocity_verlet = velocity_verlet
+isokinetic_mclachlan = mclachlan
+isokinetic_yoshida = yoshida
+isokinetic_omelyan = omelyan
+
 
 def as_coefficients(integrator):
     """Accepts one of the tables above (or any odd-length palindromic sequence of 3..11 floats)."""
     if isinstance(integrator, str):
         try:
             integrator = {"velocity_verlet": velocity_verlet, "mclachlan": mclachlan, "yoshida": yoshida,
-                          "omelyan": omelyan}[integrator]
+                          "omelyan": omelyan, "isokinetic_velocity_verlet": velocity_verlet,
+                          "isokinetic_mclachlan": mclachlan, "isokinetic_yoshida": yoshida,
+                          "isokinetic_omelyan": omelyan}[integrator]
         except KeyError:
             raise ValueError(f"unknown integrator {integrator!r}") from None
     coef = tuple(float(c) for c in integrator)

@@ -140,6 +140,7 @@ PREBUILT = (
     ("rosenbrock", 5, False, False), ("rosenbrock", 100, False, False), ("rosenbrock", 70, False, False),
     ("rosenbrock", 256, False, False), ("rosenbrock", 1024, False, False),   # SC_S1, V1, S4, V2, V8
     ("diag_gaussian_big", 2048, False, False), ("hier_logit_big", 1504, False, False),   # CTA-per-chain rows (SC_BIG)
+    ("bounded_gaussian", 2, False, True),   # SC_S1: MCLMC's NaN handling (a box whose overshoots give NaN log-densities)
 )
 
 

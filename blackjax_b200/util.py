@@ -54,6 +54,36 @@ def sample_nuts_native(rng_key, state, logdensity_fn, step_size, inverse_mass_ma
     return HMCState(q, logp, g), hist, acc, n_int
 
 
+def sample_mclmc_native(rng_key, state, logdensity_fn, L, step_size, num_steps, *, inverse_mass_matrix=1.0,
+                        integrator="isokinetic_mclachlan", desired_energy_var_max_ratio=float("inf"),
+                        desired_energy_var=5e-4, thin=1, keep_history=True, chain_offset=0):
+    """``run_inference_algorithm`` for MCLMC without a Python-level loop (libbjx ``bjx_mclmc_sample``): same draws as
+    ``num_steps`` calls of ``mclmc.step(split(rng_key, T)[t], .)``.  Returns (final IntegratorState, positions
+    [num_steps // thin, C, D] or None, energy changes [num_steps, C])."""
+    from ._engine import get_engine
+    from ._lib import check, lib, ptr
+    from .mcmc import integrators
+    from .mcmc.hmc import IntegratorState
+    from .mcmc.mclmc import energy_cutoff, metric_tensor
+    q, p, logp, g = (t.clone() for t in state)
+    eng = get_engine(q, logdensity_fn)
+    eng.set_integrator(integrators.as_coefficients(integrator))
+    eng.ensure_metric(metric_tensor(eng, inverse_mass_matrix), diagonal_only=True)
+    key = rng_key.to(q.device).contiguous()
+    if key.ndim != 1:
+        raise ValueError("sample_mclmc_native takes ONE rng_key of shape [2]")
+    eng._key_mode(key, chain_offset)
+    C, D = q.shape
+    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
+    de = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    eps, eps_dev = eng._eps(step_size)
+    L, L_dev = eng._eps(L, "L")
+    check(lib().bjx_mclmc_sample(eng.h, ptr(key), ptr(q), ptr(p), ptr(logp), ptr(g), eps, ptr(eps_dev), L, ptr(L_dev),
+                                 energy_cutoff(D, desired_energy_var_max_ratio, desired_energy_var), int(num_steps),
+                                 ptr(hist), int(thin), ptr(de)), eng.h)
+    return IntegratorState(q, p, logp, g), hist, de
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

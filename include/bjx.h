@@ -271,6 +271,32 @@ int bjx_nuts_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* lo
 /* doubling launches and the deepest tree of the last bjx_nuts_step (host ints; reading the depth synchronises the stream) */
 int bjx_nuts_last_stats(bjx_handle_t h, int64_t* doubling_launches, int64_t* depth_reached);
 
+/* ---- MCLMC: the microcanonical Langevin sampler (blackjax/mcmc/mclmc.py) -------------------------------------------
+ * State (q [C,D], p [C,D], logp [C], grad [C,D]); p is the unit-norm momentum of the whitened frame.  The metric must be
+ * BJX_METRIC_DIAG or BJX_METRIC_DIAG_PER_CHAIN (the preconditioner is sqrt(M^-1), integrators.py:437-439); the integrator is
+ * the handle's coefficient table run as the isokinetic integrator (isokinetic_mclachlan = the mclachlan table,
+ * integrators.py:533-539).  Built for 2 <= dim <= 1024 (dense Gaussian target: dim <= 128); everything else returns
+ * BJX_E_UNSUPPORTED.  Keys follow bjx_set_key_mode. */
+typedef struct {
+  float* kinetic_change; /* [C] MCLMCInfo.kinetic_change (0 on a reverted transition) */
+  float* energy_change;  /* [C] kinetic_change - logp_new + logp_old (0 on a reverted transition) */
+  uint8_t* nonans;       /* [C] 1 when q, p and logp came out finite */
+} bjx_mclmc_info;
+/* mclmc.init (mclmc.py:55-66): logp, grad = value_and_grad(q); p = generate_unit_vector(key) (util.py:94-113) */
+int bjx_mclmc_init(bjx_handle_t h, const uint32_t* keys, const float* q, float* logp_out, float* grad_out, float* p_out);
+/* mclmc.build_kernel(...).kernel (mclmc.py:104-143), in place on (q, p, logp, grad).  step_size_dev / L_dev ([C], optional)
+ * override step_size / L; L = inf leaves the momentum unrefreshed.  energy_cutoff = sqrt(dim * desired_energy_var_max_ratio *
+ * desired_energy_var) (inf by default): a transition with |energy_change| above it, or with a non-finite q, p or logp, keeps
+ * (q, logp, grad) and draws a fresh unit momentum (handle_high_energy / handle_nans, mclmc.py:215-281). */
+int bjx_mclmc_step(bjx_handle_t h, const uint32_t* keys, float* q, float* p, float* logp, float* grad, float step_size,
+                   const float* step_size_dev, float L, const float* L_dev, float energy_cutoff, const bjx_mclmc_info* info);
+/* run_inference_algorithm (util.py:150-213) for MCLMC, like bjx_hmc_sample: step keys = split(rng_key, num_steps), chain c
+ * of step t uses split(step_key_t, n_global)[chain_offset + c], no host synchronisation.  history (optional) float32
+ * [num_steps / thin, C, D]; energy_change_history (optional) float32 [num_steps, C]. */
+int bjx_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* p, float* logp, float* grad, float step_size,
+                     const float* step_size_dev, float L, const float* L_dev, float energy_cutoff, int32_t num_steps,
+                     float* history, int32_t thin, float* energy_change_history);
+
 /* ---- PRNG (jax.random restated; keys raw uint32 pairs) ----------------------------------------- */
 /* h may be NULL for the PRNG entry points: current device, and the stream this thread registered with
  * bjx_set_default_stream (a cudaStream_t; the legacy default stream until one is registered) */
