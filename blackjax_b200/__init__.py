@@ -19,7 +19,10 @@ from .mcmc import nuts as _nuts
 from .mcmc import dynamic_hmc as _dynamic_hmc
 from .mcmc import ghmc as _ghmc
 from .mcmc import mclmc as _mclmc
+from .mcmc import adjusted_mclmc as _adjusted_mclmc
+from .mcmc import adjusted_mclmc_dynamic as _adjusted_mclmc_dynamic
 from .util import run_inference_algorithm, sample_hmc_native, sample_mclmc_native, sample_nuts_native  # noqa: F401
+from .util import sample_adjusted_mclmc_native  # noqa: F401
 
 hmc = GenerateSamplingAPI(_hmc.as_top_level_api, _hmc.init, _hmc.build_kernel)     # blackjax/__init__.py:111
 nuts = GenerateSamplingAPI(_nuts.as_top_level_api, _nuts.init, _nuts.build_kernel)  # blackjax/__init__.py:112
@@ -39,5 +42,9 @@ dmhmc = GenerateSamplingAPI(                                                    
 
 ghmc = GenerateSamplingAPI(_ghmc.as_top_level_api, _ghmc.init, _ghmc.build_kernel)   # blackjax/__init__.py:139
 mclmc = GenerateSamplingAPI(_mclmc.as_top_level_api, _mclmc.init, _mclmc.build_kernel)  # blackjax/__init__.py:141
+adjusted_mclmc = GenerateSamplingAPI(_adjusted_mclmc.as_top_level_api, _adjusted_mclmc.init,
+                                     _adjusted_mclmc.build_kernel)
+adjusted_mclmc_dynamic = GenerateSamplingAPI(_adjusted_mclmc_dynamic.as_top_level_api, _adjusted_mclmc_dynamic.init,
+                                             _adjusted_mclmc_dynamic.build_kernel)
 
 __version__ = "0.1.0"

@@ -281,6 +281,34 @@ class Engine:
                                    float(energy_cutoff), C.byref(info)), self.h)
         self._mclmc_keepalive = (eps_dev, L_dev)  # the launch is asynchronous
 
+    def adjusted_mclmc_step(self, keys, q, logp, g, step_size, num_integration_steps, L_proposal_factor, out=None,
+                            info_fields=None, chain_offset=0):
+        """One adjusted MCLMC transition; ``num_integration_steps`` is an int or an int32 tensor [C] (one per chain)."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        g = _f32(g, (self.C, self.D), "logdensity_grad")
+        logp = _f32(logp, (self.C,), "logdensity")
+        qo, lo, go = out if out is not None else (torch.empty_like(q), torch.empty_like(logp), torch.empty_like(g))
+        eps, eps_dev = self._eps(step_size)
+        info = self._info(info_fields or {})
+        steps_dev = None
+        if isinstance(num_integration_steps, torch.Tensor):  # adjusted_mclmc_dynamic: one step count per chain
+            steps_dev = num_integration_steps.to(device=self.device, dtype=torch.int32).contiguous()
+            if steps_dev.shape != (self.C,):
+                raise ValueError(f"per-chain num_integration_steps must have shape ({self.C},)")
+            num_integration_steps = 0
+        check(lib().bjx_set_integration_steps(self.h, ptr(steps_dev)), self.h)
+        try:
+            check(lib().bjx_adjusted_mclmc_step(self.h, ptr(keys), ptr(q), ptr(logp), ptr(g), ptr(qo), ptr(lo), ptr(go),
+                                                eps, ptr(eps_dev), int(num_integration_steps), float(L_proposal_factor),
+                                                C.byref(info)), self.h)
+        finally:
+            if steps_dev is not None:
+                check(lib().bjx_set_integration_steps(self.h, None), self.h)
+        self._amclmc_keepalive = (steps_dev, eps_dev)  # the launch is asynchronous: keep the arrays until the next call
+        return qo, lo, go
+
     def nuts_last_stats(self):
         a, b = C.c_int64(), C.c_int64()
         check(lib().bjx_nuts_last_stats(self.h, C.byref(a), C.byref(b)), self.h)

@@ -9,6 +9,7 @@ LIB_PATH = os.path.join(_HERE, "libbjx.so")
 TARGET_DIAG_GAUSSIAN, TARGET_FUNNEL, TARGET_DENSE_GAUSSIAN, TARGET_BANANA, TARGET_HIER_LOGIT, TARGET_USER = 0, 1, 2, 3, 4, 5
 METRIC_DIAG, METRIC_DENSE, METRIC_DIAG_PER_CHAIN, METRIC_LOW_RANK, METRIC_DENSE_PER_CHAIN = 0, 1, 2, 3, 4
 CHEES_WHITEN, CHEES_LENGTH_FLOOR = 1, 2
+AMCLMC_STEPS_FIXED, AMCLMC_STEPS_RANDINT, AMCLMC_STEPS_UNIFORM = 0, 1, 2
 
 _f32p = C.c_void_p  # device pointers travel as integers
 
@@ -76,6 +77,11 @@ _SIGNATURES = {
                                  C.c_float, C.POINTER(MclmcInfo)]),
     "bjx_mclmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, _f32p,
                                    C.c_float, C.c_int32, _f32p, C.c_int32, _f32p]),
+    "bjx_adjusted_mclmc_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
+                                          C.c_int32, C.c_float, C.POINTER(Info)]),
+    "bjx_adjusted_mclmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, C.c_int32,
+                                            C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_int32, _f32p, C.c_int32, _f32p,
+                                            C.c_void_p]),
     "bjx_nuts_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
                                 C.c_int32, C.POINTER(Info), _f32p, _f32p]),
     "bjx_nuts_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, C.c_int32, _f32p,

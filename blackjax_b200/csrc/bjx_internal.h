@@ -59,3 +59,5 @@ int check_ready(bjx_handle_t h, bool need_metric, const void* const* ptrs, int n
 int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps);
 // history row (t + 1) / thin - 1 = q after transition t, when (t + 1) % thin == 0
 int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q);
+// bjx_mclmc.cu: dim >= 2, a diagonal metric and the row kernels, or BJX_E_UNSUPPORTED with "<name> ..." as the reason
+int mclmc_transition_supported(bjx_handle_t h, const char* name);

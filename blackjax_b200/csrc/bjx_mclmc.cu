@@ -24,10 +24,24 @@ static __global__ void k_unit_vector(Params P, const uint32_t* __restrict__ keys
   for (int e = lane; e < P.D; e += 32) row[e] = __fdiv_rn(row[e], n);
 }
 
-// The configurations the MCLMC kernel is built for; BJX_E_UNSUPPORTED with the reason otherwise.
-static int mclmc_supported(bjx_handle_t h) {
+// The dimensions the MCLMC kernels are built for; BJX_E_UNSUPPORTED with the reason otherwise.
+static int mclmc_supported(bjx_handle_t h, const std::string& name = "MCLMC") {
   if (h->cfg.dim < 2)
-    return bjx_fail(h, BJX_E_UNSUPPORTED, "MCLMC needs dim >= 2 (the target distribution must have more than 1 dimension)");
+    return bjx_fail(h, BJX_E_UNSUPPORTED, name + " needs dim >= 2 (the target distribution must have more than 1 dimension)");
+  return 0;
+}
+
+int mclmc_transition_supported(bjx_handle_t h, const char* name) {
+  const std::string n(name);
+  int rc = mclmc_supported(h, n);
+  if (rc) return rc;
+  if (h->metric_kind != BJX_METRIC_DIAG && h->metric_kind != BJX_METRIC_DIAG_PER_CHAIN)
+    return bjx_fail(h, BJX_E_UNSUPPORTED, n + " is built for diagonal metrics ([dim] or per-chain [n_chains, dim])");
+  switch (transition_route(h)) {
+    case ROUTE_DENSE: return bjx_fail(h, BJX_E_UNSUPPORTED, n + " with a dense Gaussian target is built for dim <= 128");
+    case ROUTE_BIG: return bjx_fail(h, BJX_E_UNSUPPORTED, n + " is built for dim <= 1024 (the warp-per-chain kernels)");
+    case ROUTE_ROWS: break;
+  }
   return 0;
 }
 
@@ -52,14 +66,7 @@ extern "C" int bjx_mclmc_step(bjx_handle_t h, const uint32_t* keys, float* q, fl
   int rc = check_ready(h, true, ptrs, 3);
   if (rc) return rc;
   if (!keys || !logp) return bjx_fail(h, BJX_E_INVALID, "null argument");
-  if ((rc = mclmc_supported(h))) return rc;
-  if (h->metric_kind != BJX_METRIC_DIAG && h->metric_kind != BJX_METRIC_DIAG_PER_CHAIN)
-    return bjx_fail(h, BJX_E_UNSUPPORTED, "MCLMC is built for diagonal metrics ([dim] or per-chain [n_chains, dim])");
-  switch (transition_route(h)) {
-    case ROUTE_DENSE: return bjx_fail(h, BJX_E_UNSUPPORTED, "MCLMC with a dense Gaussian target is built for dim <= 128");
-    case ROUTE_BIG: return bjx_fail(h, BJX_E_UNSUPPORTED, "MCLMC is built for dim <= 1024 (the warp-per-chain kernels)");
-    case ROUTE_ROWS: break;
-  }
+  if ((rc = mclmc_transition_supported(h, "MCLMC"))) return rc;
   LaunchArgs a{};
   a.P = make_params(h, step_size, step_size_dev);
   a.keys = keys;

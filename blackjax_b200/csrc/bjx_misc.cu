@@ -33,23 +33,14 @@ __global__ void k_prng_draw(const uint32_t* __restrict__ keys, long long n_keys,
   if (MODE == 2) reinterpret_cast<float*>(out)[t] = normal_at(key, i);
 }
 
-// jax.random.randint for int32 (jax/_src/random.py _randint): k1, k2 = split(key); higher/lower = random_bits(k1/k2);
-// span = maxval - minval (1 when maxval <= minval); multiplier = ((2^16 % span)^2) % span = 2^32 % span;
-// offset = ((higher % span) * multiplier + lower % span) % span, all in uint32; result = minval + offset.
+// jax.random.randint for int32 (randint_at, bjx_prng.cuh)
 __global__ void k_prng_randint(const uint32_t* __restrict__ keys, long long n_keys, long long per_key, int minval,
                                int maxval, int* __restrict__ out) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n_keys * per_key) return;
   const long long k = t / per_key;
-  const uint32_t i = (uint32_t)(t % per_key);
   const Key key{keys[2 * k], keys[2 * k + 1]};
-  const uint32_t hi = random_bits(fold_in(key, 0u), i), lo = random_bits(fold_in(key, 1u), i);
-  uint32_t span = (uint32_t)maxval - (uint32_t)minval;
-  if (maxval <= minval) span = 1u;
-  uint32_t mult = (1u << 16) % span;
-  mult = (mult * mult) % span;
-  const uint32_t off = ((hi % span) * mult + lo % span) % span;
-  out[t] = (int)((uint32_t)minval + off);
+  out[t] = randint_at(key, (uint32_t)(t % per_key), minval, maxval);
 }
 
 static inline dim3 grid1d(long long n, int b = 256) { return dim3((unsigned)((n + b - 1) / b)); }

@@ -54,6 +54,19 @@ __host__ __device__ __forceinline__ uint32_t random_bits(Key k, uint32_t i) {
   return a ^ b;
 }
 
+// jax.random.randint(key, shape, minval, maxval)[i] for int32 (jax/_src/random.py _randint): k1, k2 = split(key);
+// higher / lower = random_bits(k1 / k2); span = maxval - minval (1 when maxval <= minval); multiplier =
+// ((2^16 % span)^2) % span = 2^32 % span; offset = ((higher % span) * multiplier + lower % span) % span, all in uint32.
+__host__ __device__ __forceinline__ int randint_at(Key key, uint32_t i, int minval, int maxval) {
+  const uint32_t hi = random_bits(fold_in(key, 0u), i), lo = random_bits(fold_in(key, 1u), i);
+  uint32_t span = (uint32_t)maxval - (uint32_t)minval;
+  if (maxval <= minval) span = 1u;
+  uint32_t mult = (1u << 16) % span;
+  mult = (mult * mult) % span;
+  const uint32_t off = ((hi % span) * mult + lo % span) % span;
+  return (int)((uint32_t)minval + off);
+}
+
 __device__ __forceinline__ float bits_to_unit(uint32_t bits) {
   return __fsub_rn(__uint_as_float((bits >> 9) | 0x3F800000u), 1.0f);  // [0,1)
 }

@@ -84,6 +84,68 @@ def sample_mclmc_native(rng_key, state, logdensity_fn, L, step_size, num_steps, 
     return IntegratorState(q, p, logp, g), hist, de
 
 
+def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_steps, *, num_integration_steps=None,
+                                 integration_steps_fn=None, integration_steps_params=(), L_proposal_factor=float("inf"),
+                                 inverse_mass_matrix=1.0, integrator="isokinetic_mclachlan", divergence_threshold=1000,
+                                 thin=1, keep_history=True, chain_offset=0):
+    """``run_inference_algorithm`` for adjusted MCLMC without a Python-level loop (libbjx ``bjx_adjusted_mclmc_sample``):
+    same draws as ``num_steps`` calls of the step API with keys ``split(rng_key, T)[t]``.
+
+    Static (``adjusted_mclmc``): ``state`` is an HMCState and ``num_integration_steps`` an int.  Dynamic
+    (``adjusted_mclmc_dynamic``): ``state`` is a DynamicHMCState and ``integration_steps_fn`` one of the rules evaluated on
+    the device -- the default ``randint(key, (), 1, 10)`` or ``make_random_trajectory_length_fn(...)`` with
+    ``integration_steps_params = (avg_num_integration_steps,)``; ``random_generator_arg`` advances to ``split(key)[1]`` per
+    transition.  Other step-count functions go through the step API.  Returns (final state, positions
+    [num_steps // thin, C, D] or None, acceptance rates [num_steps, C], step counts int32 [num_steps, C])."""
+    from ._engine import get_engine
+    from ._lib import AMCLMC_STEPS_FIXED, AMCLMC_STEPS_UNIFORM, check, lib, ptr
+    from .mcmc import adjusted_mclmc_dynamic, integrators
+    from .mcmc.dynamic_hmc import DynamicHMCState
+    from .mcmc.hmc import HMCState
+    from .mcmc.mclmc import metric_tensor
+    dynamic = isinstance(state, DynamicHMCState)
+    rule, min_steps, n, scale, rga = AMCLMC_STEPS_FIXED, 0, 0, 0.0, None
+    if dynamic:
+        fn = integration_steps_fn or adjusted_mclmc_dynamic._integration_steps
+        if getattr(fn, "device_rule", None) is None:
+            raise ValueError("sample_adjusted_mclmc_native evaluates the default randint rule and "
+                             "make_random_trajectory_length_fn(...) on the device; use the step API for other "
+                             "integration_steps_fn")
+        rule, min_steps = fn.device_rule
+        if rule == AMCLMC_STEPS_FIXED:
+            n = fn(None, *integration_steps_params)
+        elif rule == AMCLMC_STEPS_UNIFORM:
+            (avg,) = integration_steps_params
+            scale = float(adjusted_mclmc_dynamic.rescale(avg))
+        q, logp, g, rga = (t.clone() for t in state)
+        if rga.dtype not in (torch.uint32, torch.int32) or tuple(rga.shape) != (q.shape[0], 2):
+            raise ValueError("random_generator_arg must be uint32 [n_chains, 2]")
+        rga = rga.contiguous()
+    else:
+        if num_integration_steps is None:
+            raise ValueError("the static sampler needs num_integration_steps")
+        from .mcmc.adjusted_mclmc import steps_argument
+        n = steps_argument(num_integration_steps)
+        q, logp, g = (t.clone() for t in state)
+    eng = get_engine(q, logdensity_fn, divergence_threshold=divergence_threshold)
+    eng.set_integrator(integrators.as_coefficients(integrator))
+    eng.ensure_metric(metric_tensor(eng, inverse_mass_matrix), diagonal_only=True)
+    key = rng_key.to(q.device).contiguous()
+    if key.ndim != 1:
+        raise ValueError("sample_adjusted_mclmc_native takes ONE rng_key of shape [2]")
+    eng._key_mode(key, chain_offset)
+    C, D = q.shape
+    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
+    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    steps = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    eps, eps_dev = eng._eps(step_size)
+    check(lib().bjx_adjusted_mclmc_sample(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev),
+                                          float(L_proposal_factor), int(rule), int(n), scale, int(min_steps), ptr(rga),
+                                          int(num_steps), ptr(hist), int(thin), ptr(acc), ptr(steps)), eng.h)
+    final = DynamicHMCState(q, logp, g, rga) if dynamic else HMCState(q, logp, g)
+    return final, hist, acc, steps
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

@@ -297,6 +297,39 @@ int bjx_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* p
                      const float* step_size_dev, float L, const float* L_dev, float energy_cutoff, int32_t num_steps,
                      float* history, int32_t thin, float* energy_change_history);
 
+/* ---- Adjusted MCLMC / MAMS: the Metropolis-adjusted microcanonical sampler (blackjax/mcmc/adjusted_mclmc.py,
+ * adjusted_mclmc_dynamic.py) ----------------------------------------------------------------------------------------
+ * State (q [C,D], logp [C], grad [C,D]) as HMC's; initialise it with bjx_init_state.  One transition draws a unit momentum
+ * from split(key)[0], runs num_integration_steps steps of the handle's coefficient table as the isokinetic integrator, each
+ * between two partial momentum refreshes with L_proposal = L_proposal_factor * num_integration_steps * step_size (none when
+ * L_proposal_factor = inf), and accepts with Metropolis-Hastings; there is no momentum flip.  Per-chain step counts come from
+ * bjx_set_integration_steps (adjusted_mclmc_dynamic); 0 steps is allowed and accepts the unchanged state.  bjx_info as HMCInfo:
+ * energy = -logp of the proposal, momentum = the drawn unit vector, proposal_momentum = the unflipped end momentum.
+ * Same support as MCLMC: diagonal metrics, 2 <= dim <= 1024 (dense Gaussian target: dim <= 128), else BJX_E_UNSUPPORTED.
+ * Keys follow bjx_set_key_mode.  A rejected in-place transition writes nothing. */
+int bjx_adjusted_mclmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in,
+                            const float* grad_in, float* q_out, float* logp_out, float* grad_out, float step_size,
+                            const float* step_size_dev, int32_t num_integration_steps, float L_proposal_factor,
+                            const bjx_info* info);
+/* Step-count rules of bjx_adjusted_mclmc_sample, evaluated on the device from each chain's random_generator_arg key, which
+ * then advances to split(key)[1] (adjusted_mclmc_dynamic.py:58,124):
+ *   BJX_AMCLMC_STEPS_FIXED    num_integration_steps for every chain (adjusted_mclmc), random_generator_arg unused;
+ *   BJX_AMCLMC_STEPS_RANDINT  jax.random.randint(key, (), 1, 10) (adjusted_mclmc_dynamic.py:55);
+ *   BJX_AMCLMC_STEPS_UNIFORM  max(ceil(uniform(key) * steps_scale), min_steps), steps_scale = rescale(avg) in float32
+ *                             (adjusted_mclmc_dynamic.py:234-238 with min_steps = 1; the reference's own tests use 0). */
+#define BJX_AMCLMC_STEPS_FIXED 0
+#define BJX_AMCLMC_STEPS_RANDINT 1
+#define BJX_AMCLMC_STEPS_UNIFORM 2
+/* run_inference_algorithm (util.py:150-213) for adjusted MCLMC, like bjx_hmc_sample: step keys = split(rng_key, num_steps),
+ * no host synchronisation.  random_generator_arg uint32 [C, 2] (rules other than FIXED) is advanced in place.  history
+ * (optional) float32 [num_steps / thin, C, D]; acceptance_history (optional) float32 [num_steps, C];
+ * steps_history (optional) int32 [num_steps, C]. */
+int bjx_adjusted_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, float* grad, float step_size,
+                              const float* step_size_dev, float L_proposal_factor, int32_t steps_rule,
+                              int32_t num_integration_steps, float steps_scale, int32_t min_steps,
+                              uint32_t* random_generator_arg, int32_t num_steps, float* history, int32_t thin,
+                              float* acceptance_history, int32_t* steps_history);
+
 /* ---- PRNG (jax.random restated; keys raw uint32 pairs) ----------------------------------------- */
 /* h may be NULL for the PRNG entry points: current device, and the stream this thread registered with
  * bjx_set_default_stream (a cudaStream_t; the legacy default stream until one is registered) */
