@@ -12,6 +12,7 @@ from ._lib import BjxError  # noqa: F401
 from .adaptation.window_adaptation import build_schedule, window_adaptation  # noqa: F401
 from .adaptation.chees_adaptation import chees_adaptation  # noqa: F401
 from .adaptation.meads_adaptation import meads_adaptation  # noqa: F401
+from .adaptation.mclmc_adaptation import MCLMCAdaptationState, mclmc_find_L_and_step_size  # noqa: F401
 from .base import AdaptationAlgorithm, AdaptationResults, GenerateSamplingAPI, SamplingAlgorithm  # noqa: F401
 from . import mcmc  # noqa: F401
 from .mcmc import hmc as _hmc

@@ -77,6 +77,13 @@ _SIGNATURES = {
                                  C.c_float, C.POINTER(MclmcInfo)]),
     "bjx_mclmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, _f32p,
                                    C.c_float, C.c_int32, _f32p, C.c_int32, _f32p]),
+    "bjx_mclmc_tune_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float,
+                                      _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32, C.c_double, C.c_double, C.c_double,
+                                      C.c_void_p]),
+    "bjx_mclmc_ess_per_chain": (C.c_int, [C.c_void_p, _f32p, C.c_int32, _f32p, C.c_void_p]),
+    "bjx_mclmc_find_l_and_step_size": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                                 C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                                 C.c_double, C.c_double, C.c_double, C.c_double, C.c_int64, C.c_void_p]),
     "bjx_adjusted_mclmc_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
                                           C.c_int32, C.c_float, C.POINTER(Info)]),
     "bjx_adjusted_mclmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, C.c_int32,

@@ -29,6 +29,8 @@ void launch_prng_randint(const uint32_t* keys, long long n, long long per_key, i
                          cudaStream_t s);
 size_t ess_scratch_floats(int T, int C, int D);
 void launch_ess(int T, int C, int D, const float* hist, float* ess, float* scratch, cudaStream_t s);
+// single-chain ESS of every (chain, dim) series: ess [C, D]; lags_out (optional, zeroed) [C] lags evaluated per chain
+void launch_ess_per_chain(int T, int C, int D, const float* hist, float* ess, int* lags_out, cudaStream_t s);
 // windowed D x D covariance accumulators of bjx_adapt.cu: cov_stat_blocks(C) blocks of cov_block_floats(D) floats (count,
 // -, mean[D], m2[D, D] lower triangle); the fold uses nb * (2 + 2D) floats of stats scratch; the merge writes the full
 // covariance m2 / max(n - 1, 1) [D, D] to out and (n, mean[D]) to count_mean

@@ -530,6 +530,115 @@ void launch_ess(int T, int C, int D, const float* hist, float* ess, float* scrat
   k_ess_finish<<<(D + 127) / 128, 128, 0, s>>>(T, C, D, mean, has_var, acov, ess);
 }
 
+// ---- single-chain ESS of every (chain, dim) series of a history [T, C, D] -----------------------------------------------
+// effective_sample_size(history[:, c, None, :]) for every chain c (mclmc_adaptation.py:393): the arithmetic of k_ess_chain_mean,
+// k_ess_autocov and k_ess_finish with C = 1, but a thread owns one series from its mean to its ESS.  Geyer's procedure reads
+// the autocorrelation only up to the pair after the initial positive sequence, so the warp (32 dims of one chain) evaluates
+// blocks of kEssLags lags, feeding each pair into the sequence as it arrives, until every series of the warp has ended its
+// initial positive sequence and seen that next pair.  Each lag's sum is the same fmaf chain as k_ess_autocov's, and the
+// pairs go through the same operations in the same order as k_ess_finish, so the result is that of evaluating all lags.
+// lags_out (optional, zeroed by the caller): per chain, the most lags any of its warps evaluated.
+__global__ void __launch_bounds__(128) k_ess_chain(int T, int C, int D, const float* __restrict__ hist, float* __restrict__ ess,
+                                                   int* __restrict__ lags_out) {
+  const int lane = threadIdx.x & 31;
+  const int d_blocks = (D + 31) / 32;
+  const long long w = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w >= (long long)C * d_blocks) return;
+  const int c = (int)(w / d_blocks);
+  const int d = (int)(w % d_blocks) * 32 + lane;
+  const bool live = d < D;
+  const size_t CD = (size_t)C * D;
+  const float* series = hist + (size_t)c * D + (live ? d : 0);
+  // k_ess_chain_mean
+  float m = 0.f;
+  bool varies = false;
+  if (live) {
+    const float x0 = series[0];
+    double acc = 0.0;
+    for (int i = 0; i < T; ++i) {
+      const float x = series[(size_t)i * CD];
+      acc += (double)x;
+      varies |= (x != x0);
+    }
+    m = (float)(acc / (double)T);
+  }
+  auto at = [&](int s) -> float { return (live && s < T) ? series[(size_t)s * CD] - m : 0.f; };
+  const double norm = 1.0 / ((double)T * 1.0);
+  const float Tf = (float)T;
+  const int K = (T - T % 2) / 2;
+  float var0 = 0.f, wvar = 1.f, carry = 0.f, sum = 0.f, e_at = 0.f;
+  bool degenerate = false, done = !live;
+  int lag0 = 0;
+  for (;; lag0 += kEssLags) {
+    // k_ess_autocov for lags lag0 .. lag0 + kEssLags - 1
+    float acc[kEssLags];
+#pragma unroll
+    for (int l = 0; l < kEssLags; ++l) acc[l] = 0.f;
+    float a[kEssDraws], win[kEssLags + kEssDraws];
+#pragma unroll
+    for (int i = 0; i < kEssLags; ++i) win[i] = at(lag0 + i);
+    for (int s = 0; s < T - lag0; s += kEssDraws) {
+#pragma unroll
+      for (int i = 0; i < kEssDraws; ++i) {
+        a[i] = at(s + i);
+        win[kEssLags + i] = at(s + lag0 + kEssLags + i);
+      }
+#pragma unroll
+      for (int i = 0; i < kEssDraws; ++i) {
+#pragma unroll
+        for (int l = 0; l < kEssLags; ++l) acc[l] = fmaf(a[i], win[i + l], acc[l]);
+      }
+#pragma unroll
+      for (int i = 0; i < kEssLags; ++i) win[i] = win[i + kEssDraws];
+    }
+    if (lag0 == 0) {  // k_ess_finish :222-240 with C = 1
+      var0 = (float)((double)acc[0] * norm) * Tf / (Tf - 1.0f);
+      degenerate = isfinite(var0) && (!varies || var0 <= 0.0f);
+      wvar = var0 * (Tf - 1.0f) / Tf;
+      if (degenerate) wvar = 1.0f;
+    }
+    // pairs lag0 / 2 .. lag0 / 2 + kEssLags / 2 - 1 through Geyer's initial positive and monotone sequences (:243-297)
+#pragma unroll
+    for (int p = 0; p < kEssLags / 2; ++p) {
+      const int k = lag0 / 2 + p;
+      if (!done && k < K) {
+        const float re = (k == 0) ? 1.0f : 1.0f - (var0 - (float)((double)acc[2 * p] * norm)) / wvar;
+        const float ro = 1.0f - (var0 - (float)((double)acc[2 * p + 1] * norm)) / wvar;
+        const bool positive = re + ro > 0.0f;
+        if (!positive && k == 0) {  // no positive pair: every pair is masked to zero
+          done = true;
+        } else {
+          // in the sequence: (re, ro); the pair after it (k == max_t + 1): its even term when positive, no odd term
+          float e = positive ? re : (re > 0.0f ? re : 0.f);
+          float o = positive ? ro : 0.f;
+          const float sp = e + o;
+          if (k == 0) carry = sp;
+          const bool upd = sp > carry;
+          const float nxt = upd ? carry : sp;
+          carry = nxt;
+          if (upd) e = o = nxt / 2.0f;
+          sum += e + o;
+          e_at = e;  // idx_get is the pair after the sequence, or the last pair when every pair is positive
+          done = !positive;
+        }
+      }
+    }
+    if (lag0 + kEssLags >= 2 * K) done = true;  // every pair seen
+    if (__all_sync(0xffffffffu, done)) break;
+  }
+  if (lags_out && lane == 0) atomicMax(lags_out + c, min(lag0 + kEssLags, T));
+  if (!live) return;
+  const float ess_raw = 1.0f * (float)T;                                           // :292
+  float tau = -1.0f + 2.0f * sum - e_at;                                           // :293-297
+  tau = fmaxf(tau, 1.0f / log10f(ess_raw));                                        // :299
+  ess[(size_t)c * D + d] = degenerate ? 0.0f : ess_raw / tau;                      // :300-301
+}
+
+void launch_ess_per_chain(int T, int C, int D, const float* hist, float* ess, int* lags_out, cudaStream_t s) {
+  const long long warps = (long long)C * ((D + 31) / 32);
+  k_ess_chain<<<(unsigned)((warps + 3) / 4), 128, 0, s>>>(T, C, D, hist, ess, lags_out);
+}
+
 void launch_pooled_stats(int C, int D, const float* x, const float* acc, float* out, cudaStream_t s) {
   k_pooled_accept<<<1, 1024, 0, s>>>(C, acc, out);
   k_pooled_colstats<<<dim3((D + 31) / 32), dim3(32, 8), 0, s>>>(C, D, x, out);

@@ -21,10 +21,13 @@ def potential_scale_reduction(history, logdensity_fn):
     return rhat
 
 
-def effective_sample_size(history, logdensity_fn):
+def effective_sample_size(history, logdensity_fn, per_chain=False):
     """``blackjax.diagnostics.effective_sample_size`` (blackjax/diagnostics.py:159-305) for ``history`` of shape
     [num_samples, n_chains, dim]: ESS per dimension (Geyer's initial positive / monotone sequence estimators on the
-    chain-averaged autocovariance, evaluated on the device).  ``logdensity_fn`` only selects the engine."""
+    chain-averaged autocovariance, evaluated on the device).  ``logdensity_fn`` only selects the engine.
+
+    ``per_chain=True``: the single-chain ESS of every chain, ``effective_sample_size(history[:, c, None, :])`` for each
+    c, as an [n_chains, dim] tensor (the estimate MCLMC's tuner uses)."""
     from ._engine import get_engine
     if history.ndim != 3:
         raise ValueError("history must have shape [num_samples, n_chains, dim]")
@@ -32,6 +35,10 @@ def effective_sample_size(history, logdensity_fn):
     assert T > 1, f"The input array must have at least 2 samples, got only {T}."
     history = history.contiguous()
     eng = get_engine(history[0], logdensity_fn)
+    if per_chain:
+        ess = torch.empty(C, D, dtype=torch.float32, device=history.device)
+        check(lib().bjx_mclmc_ess_per_chain(eng.h, ptr(history), int(T), ptr(ess), None), eng.h)
+        return ess
     ess = torch.empty(D, dtype=torch.float32, device=history.device)
     n = int(lib().bjx_ess_scratch_floats(int(T), int(C), int(D)))
     scratch = torch.empty((n + 1) // 2, dtype=torch.float64, device=history.device).view(torch.float32)

@@ -83,6 +83,11 @@ def build_kernel(integrator=isokinetic_mclachlan, desired_energy_var_max_ratio: 
         info = MCLMCInfo(logp, fields["kinetic_change"], fields["energy_change"], fields["nonans"].bool())
         return IntegratorState(q, p, logp, g), info
 
+    # what mclmc_find_L_and_step_size runs its native tuner with
+    kernel.coefficients = coefficients
+    kernel.desired_energy_var_max_ratio = desired_energy_var_max_ratio
+    kernel.desired_energy_var = desired_energy_var
+    kernel.chain_offset = chain_offset
     return kernel
 
 

@@ -297,6 +297,50 @@ int bjx_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* p
                      const float* step_size_dev, float L, const float* L_dev, float energy_cutoff, int32_t num_steps,
                      float* history, int32_t thin, float* energy_change_history);
 
+/* ---- MCLMC tuning: mclmc_find_L_and_step_size (blackjax/adaptation/mclmc_adaptation.py:42-399) -----------------------
+ * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
+ * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_mclmc_step (BJX_E_UNSUPPORTED otherwise).
+ * The tuner constants are the reference's Python floats: desired_energy_var, trust_in_estimate and num_effective_samples
+ * enter as D * desired_energy_var, 6 * trust_in_estimate and (n - 1) / (n + 1), formed in double and rounded to float32. */
+/* One tuning step (predictor + step, mclmc_adaptation.py:223-301) in place, for every chain.  keys (per bjx_set_key_mode)
+ * give each chain's step key k; (rng_key, nan_key) = split(k), and rng_key drives the transition with L / L_dev and the
+ * handle's metric.  A chain whose transition has nonans = 0 or a non-finite energy change keeps its whole previous state
+ * (momentum included, or generate_unit_vector(nan_key) when the transition's logdensity is NaN) and sets
+ * step_size_max = 0.8 step_size; otherwise it takes nan_to_num of the new state.  step_size, time, x_average and
+ * step_size_max ([C] float32, in/out) are the predictor's per-chain scalars; the new step size is
+ * (x_average / time)^(-1/6) clipped against step_size_max (0 where equal or NaN, as XLA evaluates the reference's
+ * predicate products).  With mask = 1, total [C] and moments [C, 2, D] (in/out; 16-byte aligned) take the streaming
+ * average of (x, x^2) with weight success * new step size (incremental_value_update, util.py:287-319); with mask = 0 or
+ * moments NULL neither is touched.  success (optional) [C] uint8. */
+int bjx_mclmc_tune_step(bjx_handle_t h, const uint32_t* keys, float* q, float* p, float* logp, float* grad, float* step_size,
+                        float L, const float* L_dev, float energy_cutoff, float* time, float* x_average, float* step_size_max,
+                        float* total, float* moments, int32_t mask, double desired_energy_var, double trust_in_estimate,
+                        double num_effective_samples, uint8_t* success);
+/* effective_sample_size(history[:, c, None, :]) for every chain: history float32 [num_samples, C, D] (C, D of the handle),
+ * ess_out [C, D] single-chain ESS.  Evaluates the autocovariance only up to the lags Geyer's initial positive sequence
+ * reads, with the result of evaluating all of them.  lags_evaluated (optional) [C]: the most lags any series of the chain
+ * needed, in blocks of 32.  Needs no scratch. */
+int bjx_mclmc_ess_per_chain(bjx_handle_t h, const float* history, int32_t num_samples, float* ess_out, int32_t* lags_evaluated);
+/* mclmc_find_L_and_step_size, all three stages on the handle's stream with no host synchronisation.  rng_key per
+ * bjx_set_key_mode: one key [2] (chain c: split(rng_key, n_global)[chain_offset + c]) or per-chain keys [C, 2].  The host
+ * computes the stage lengths: num_steps1 = round(N f1), num_steps2 = round(N f2), readjust_steps = round(num_steps2 / 3),
+ * num_steps3 = round(N f3) (Python's round).  step_size [C], L [C] and inverse_mass_matrix [C, D] (a per-chain diagonal
+ * metric, used in place of the handle's, which must still be a diagonal kind) are the initial parameters in and the tuned
+ * ones out; q, p, logp, grad the state.  Stages 1 and 2 run num_steps1 + num_steps2 tuning steps with the initial L,
+ * estimating the moments over the last num_steps2.  If num_steps2 > 1: L = sqrt(sum var), or with
+ * diagonal_preconditioning inverse_mass_matrix = var, L = sqrt(D) and readjust_steps more tuning steps (initial L, the new
+ * metric).  If num_steps3 >= 2: num_steps3 transitions with the tuned parameters and L = l_factor * step_size *
+ * mean(num_steps3 / ESS), run on slices of chains whose position history [num_steps3, slice, D] fits max_history_bytes
+ * (at least one chain); the result does not depend on the slice size.  energy_cutoff as in bjx_mclmc_step.
+ * divergence_history (optional) uint8 [num_steps1 + num_steps2 (+ readjust_steps when they run), C]: 1 where a tuning
+ * step failed (the reference's scan output). */
+int bjx_mclmc_find_l_and_step_size(bjx_handle_t h, const uint32_t* rng_key, float* q, float* p, float* logp, float* grad,
+                                   float* step_size, float* L, float* inverse_mass_matrix, int32_t num_steps1,
+                                   int32_t num_steps2, int32_t readjust_steps, int32_t num_steps3,
+                                   int32_t diagonal_preconditioning, float energy_cutoff, double desired_energy_var,
+                                   double trust_in_estimate, double num_effective_samples, double l_factor,
+                                   int64_t max_history_bytes, uint8_t* divergence_history);
+
 /* ---- Adjusted MCLMC / MAMS: the Metropolis-adjusted microcanonical sampler (blackjax/mcmc/adjusted_mclmc.py,
  * adjusted_mclmc_dynamic.py) ----------------------------------------------------------------------------------------
  * State (q [C,D], logp [C], grad [C,D]) as HMC's; initialise it with bjx_init_state.  One transition draws a unit momentum
