@@ -46,7 +46,10 @@ constexpr int kThreads = 384;            // warpgroup 0: producer; warpgroups 1-
 constexpr int kTileBytes = kBM * kBK * 2;                  // one [128 x 64] binary16 tile (kBN == kBM)
 constexpr int kStageBytes = 4 * kTileBytes;                // x1, x2, a1, a2
 constexpr int kOffBar = kStages * kStageBytes;
-constexpr int kSmemBytes = kOffBar + 2 * kStages * 8 + 1024;  // + slack to align the base to 1024
+// epilogue staging: per consumer warp 8 rows x 128 float32 of Y, rows padded by 4 floats against bank conflicts
+constexpr int kStgLd = kBN + 4;
+constexpr int kOffStg = kOffBar + 64;                      // after the 2 x kStages barriers, 16-byte aligned
+constexpr int kSmemBytes = kOffStg + 8 * 8 * kStgLd * 4 + 1024;  // + slack to align the base to 1024
 static_assert(kBN == kBM, "the operand tiles of X and A share one size");
 static_assert(kSmemBytes <= 232448, "over the 227 KB dynamic shared memory limit");
 
@@ -141,8 +144,9 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t u) { return __half22float2(
 //   warpgroups 1-2   consumers: warpgroup w owns rows [64 (w-1), +64) of the tile; per stage 3 x 4 wgmma, and once
 //                    they are issued the previous stage's group is waited for and that stage released (one arrival per
 //                    consumer warp); per tile the epilogue from the registers, its global inputs loaded before the
-//                    tile's K loop.  The producer warpgroup runs on 40 registers per thread so that the consumers
-//                    can hold those inputs beside the accumulators (232).
+//                    tile's K loop, its rows of Y staged in shared memory beside the ring and stored row by row.  The
+//                    producer warpgroup runs on 40 registers per thread so that the consumers can hold those inputs
+//                    beside the accumulators (232).
 // Accumulator fragment of m64n128 (per warp of the warpgroup): d[4j + 2h + e] is row 16 warp + 8h + lane / 4,
 // column 8j + 2 (lane % 4) + e.
 __global__ void __launch_bounds__(kThreads, 1)
@@ -206,9 +210,10 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
   for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     const int m0 = (t / tiles_n) * kBM, n0 = (t % tiles_n) * kBN;
     // Every input of this tile's epilogue is loaded here, so that the loads complete behind the K loop's MMAs and the
-    // epilogue itself only computes and stores.  Y may alias Cin, but only elementwise: element (r, c) is read as Cin and
-    // written as Y by the same thread and by no other, so reading it before the K loop reads the same value.  The per-row
-    // arrays read here (step sizes, unscales, stale maxima) are never among the same launch's outputs.
+    // epilogue itself only computes and stores.  Y may alias Cin, but only elementwise: element (r, c) is read as Cin
+    // by one thread and written as Y only by a lane of the same warp, after that thread's Cin value went into it, so
+    // reading it before the K loop reads the same value.  The per-row arrays read here (step sizes, unscales, stale
+    // maxima) are never among the same launch's outputs.
     float al_row[2], sc_row[2];
     float2 cin[2][kBN / 8];
 #pragma unroll
@@ -264,15 +269,17 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
     __syncwarp();
     if (lane == 0) mbar_arrive(empty_bar(s_prev));
 
-    // epilogue: two rows per thread, two adjacent columns per fragment register pair
+    // epilogue: two rows per thread, two adjacent columns per fragment register pair.  Y goes through this warp's
+    // staging rows in shared memory, so that every global store of the warp writes whole rows (a fragment store would
+    // touch 8 rows with 32 bytes each); the planes of Y are split from the staged rows, four columns per lane.
+    float* stg = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + kOffStg) + (warp - 4) * 8 * kStgLd;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int r = m0 + 64 * wg + 16 * wq + 8 * h + (lane >> 2);
+      const int r0 = m0 + 64 * wg + 16 * wq + 8 * h;  // the warp's 8 rows of this half
+      const int r = r0 + (lane >> 2);
       const bool live = r < M;
       const float al = al_row[h], sc = sc_row[h];
       float amax = 0.f;
-      float* yr = Y + (size_t)r * N;
-      uint16_t* pr = planes_out ? planes_out + (size_t)r * 2 * KP_out : nullptr;
 #pragma unroll
       for (int j = 0; j < kBN / 8; ++j) {
         const int c = n0 + 8 * j + 2 * (lane & 3);
@@ -291,16 +298,28 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
         } else {
           y = make_float2(al * a0, al * a1);
         }
-        *reinterpret_cast<float2*>(yr + c) = y;
+        *reinterpret_cast<float2*>(stg + (lane >> 2) * kStgLd + (c - n0)) = y;
+        if (E.planes) amax = fmaxf(amax, fmaxf(fabsf(y.x), fabsf(y.y)));
+      }
+      __syncwarp();
+      const int cw = n0 + 4 * lane;  // the four columns this lane stores of every staged row
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float sci = __shfl_sync(0xffffffffu, sc, 4 * i);
+        if (r0 + i >= M || cw >= N) continue;
+        const float4 y = *reinterpret_cast<const float4*>(stg + i * kStgLd + 4 * lane);
+        *reinterpret_cast<float4*>(Y + (size_t)(r0 + i) * N + cw) = y;
         if (E.planes) {
-          amax = fmaxf(amax, fmaxf(fabsf(y.x), fabsf(y.y)));
-          const float s0 = y.x * sc, s1 = y.y * sc;
-          const uint32_t hx = pack_h2(s0, s1);
-          const float2 f = unpack_h2(hx);
-          *reinterpret_cast<uint32_t*>(pr + c) = hx;
-          *reinterpret_cast<uint32_t*>(pr + KP_out + c) = pack_h2(s0 - f.x, s1 - f.y);
+          const float s0 = y.x * sci, s1 = y.y * sci, s2 = y.z * sci, s3 = y.w * sci;
+          const uint32_t h01 = pack_h2(s0, s1), h23 = pack_h2(s2, s3);
+          const float2 f01 = unpack_h2(h01), f23 = unpack_h2(h23);
+          uint16_t* pri = planes_out + (size_t)(r0 + i) * 2 * KP_out + cw;
+          *reinterpret_cast<uint2*>(pri) = make_uint2(h01, h23);
+          *reinterpret_cast<uint2*>(pri + KP_out) =
+              make_uint2(pack_h2(s0 - f01.x, s1 - f01.y), pack_h2(s2 - f23.x, s3 - f23.y));
         }
       }
+      __syncwarp();  // the staging rows are rewritten by the next half
       if (E.planes) {  // the four lanes of a row hold its 128 columns of this tile
         amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
         amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
