@@ -82,30 +82,62 @@ def chees_adaptation(logdensity_fn, num_chains: int, *, jitter_amount: float = 1
         dev = positions.device
         comm, n_ranks, rank = nccl_comm(dev, process_group)
         max_bits = int(math.ceil(math.log2(num_steps + max_sampling_steps)))
-        if mass_matrix_estimation == "diagonal":
-            return _run_diagonal(rng_key, positions, step_size, optim, num_steps, max_bits, comm, n_ranks, rank)
+        diagonal = mass_matrix_estimation == "diagonal"
+        L_ = lib()
+        if diagonal:
+            n_ms = L_.bjx_chees_metric_state_floats(C, D, n_ranks, options)
+            if n_ms <= 0:
+                raise ValueError("mass_matrix_estimation='diagonal' is built for dim <= 1024")
         kernel = hmc.build_kernel(full_info=True, chain_offset=rank * C)
         state = hmc.init(positions, logdensity_fn)
         eng = get_engine(positions, logdensity_fn)
-        L_ = lib()
         st = torch.empty(L_.bjx_chees_state_floats(C, D, n_ranks), dtype=torch.float32, device=dev)
         eps_c = torch.empty(C, dtype=torch.float32, device=dev)
         steps_c = torch.empty(C, dtype=torch.int32, device=dev)
         hist = torch.empty(num_steps, 4, dtype=torch.float32, device=dev)
-        imm = torch.ones(D, dtype=torch.float32, device=dev)
         check(L_.bjx_chees_init(eng.h, ptr(st), float(step_size), max_bits, float(jitter_amount), ptr(eps_c), ptr(steps_c)), eng.h)
+        hyper = (float(optim.learning_rate), float(optim.b1), float(optim.b2), float(target_acceptance_rate), float(decay_rate),
+                 int(max_leapfrog_steps))
+        if diagonal:
+            ms = torch.empty(n_ms, dtype=torch.float32, device=dev)
+            lam = torch.empty(num_steps, dtype=torch.float32, device=dev)
+            eng_flag = torch.empty(num_steps, dtype=torch.float32, device=dev)
+            imm = torch.empty(D, dtype=torch.float32, device=dev)
+            check(L_.bjx_chees_metric_init(eng.h, ptr(ms), n_ranks, options, ptr(imm)), eng.h)
+            # the update rewrites imm and re-installs it on the handle: the kernel's metric cache stays keyed on this tensor
+            eng._imm, eng._imm_key = imm, (imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device))
+            window_start = int(mass_matrix_window_fraction * num_steps)          # chees_adaptation.py:799
+            floor_on = bool(options & CHEES_LENGTH_FLOOR)
+
+            def update(t, init_q, new_q, info):
+                in_window = t >= window_start
+                recompute = floor_on and in_window and t % LENGTH_FLOOR_RECOMPUTE_INTERVAL == 0
+                return L_.bjx_chees_update_metric(eng.h, comm, n_ranks, options, ptr(st), ptr(ms), ptr(init_q),
+                                                  ptr(info.proposal.position), ptr(info.proposal.momentum), ptr(new_q),
+                                                  ptr(info.acceptance_rate), ptr(info.is_divergent.to(torch.uint8)), *hyper,
+                                                  int(in_window), int(recompute), ptr(eps_c), ptr(steps_c), ptr(hist), ptr(imm),
+                                                  ptr(lam), ptr(eng_flag))
+        else:
+            imm = torch.ones(D, dtype=torch.float32, device=dev)
+
+            def update(t, init_q, new_q, info):
+                return L_.bjx_chees_update(eng.h, comm, n_ranks, ptr(st), ptr(init_q), ptr(info.proposal.position),
+                                           ptr(info.proposal.momentum), ptr(info.acceptance_rate),
+                                           ptr(info.is_divergent.to(torch.uint8)), *hyper, ptr(eps_c), ptr(steps_c), ptr(hist))
         keys = bjx_random.split(rng_key.to(dev), num_steps)
         for t in range(num_steps):
             init_q = state.position
             state, info = kernel(keys[t], state, logdensity_fn, eps_c, imm, steps_c)
-            check(L_.bjx_chees_update(eng.h, comm, n_ranks, ptr(st), ptr(init_q), ptr(info.proposal.position),
-                                      ptr(info.proposal.momentum), ptr(info.acceptance_rate),
-                                      ptr(info.is_divergent.to(torch.uint8)), float(optim.learning_rate), float(optim.b1),
-                                      float(optim.b2), float(target_acceptance_rate), float(decay_rate),
-                                      int(max_leapfrog_steps), ptr(eps_c), ptr(steps_c), ptr(hist)), eng.h)
+            check(update(t, init_q, state.position, info), eng.h)
         import ctypes as C_
-        out = (C_.c_float * 2)()
-        check(L_.bjx_chees_final(eng.h, ptr(st), out), eng.h)          # the one host read of the warm-up
+        out = (C_.c_float * 4)()                                             # the one host read of the warm-up
+        if diagonal:
+            check(L_.bjx_chees_final_metric(eng.h, comm, n_ranks, options, ptr(st), ptr(ms), int(max_leapfrog_steps), ptr(imm),
+                                            out), eng.h)
+            imm.add_(0.0)  # version bump: later users of imm re-derive mass_matrix_sqrt from the contents the device wrote
+            eng._imm_key = (imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device))
+        else:
+            check(L_.bjx_chees_final(eng.h, ptr(st), out), eng.h)
         step, n_lf = float(out[0]), float(out[1])
         jitter = lambda i: halton_sequence(i, max_bits) * jitter_amount + (1.0 - jitter_amount)
         parameters = {
@@ -116,62 +148,8 @@ def chees_adaptation(logdensity_fn, num_chains: int, *, jitter_amount: float = 1
             "integration_steps_params": (n_lf,),
         }
         last = dynamic_hmc.DynamicHMCState(state.position, state.logdensity, state.logdensity_grad, num_steps)
+        if diagonal:
+            return AdaptationResults(last, parameters), ChEESMetricInfo(hist.cpu(), lam.cpu(), eng_flag.cpu().bool(), bool(out[2]))
         return AdaptationResults(last, parameters), hist.cpu()
-
-    def _run_diagonal(rng_key, positions, step_size, optim, num_steps, max_bits, comm, n_ranks, rank):
-        from .._engine import get_engine
-        C, D = positions.shape
-        dev = positions.device
-        kernel = hmc.build_kernel(full_info=True, chain_offset=rank * C)
-        state = hmc.init(positions, logdensity_fn)
-        eng = get_engine(positions, logdensity_fn)
-        L_ = lib()
-        st = torch.empty(L_.bjx_chees_state_floats(C, D, n_ranks), dtype=torch.float32, device=dev)
-        n_ms = L_.bjx_chees_metric_state_floats(C, D, n_ranks, options)
-        if n_ms <= 0:
-            raise ValueError("mass_matrix_estimation='diagonal' is built for dim <= 1024")
-        ms = torch.empty(n_ms, dtype=torch.float32, device=dev)
-        eps_c = torch.empty(C, dtype=torch.float32, device=dev)
-        steps_c = torch.empty(C, dtype=torch.int32, device=dev)
-        hist = torch.empty(num_steps, 4, dtype=torch.float32, device=dev)
-        lam = torch.empty(num_steps, dtype=torch.float32, device=dev)
-        eng_flag = torch.empty(num_steps, dtype=torch.float32, device=dev)
-        imm = torch.empty(D, dtype=torch.float32, device=dev)
-        check(L_.bjx_chees_init(eng.h, ptr(st), float(step_size), max_bits, float(jitter_amount), ptr(eps_c), ptr(steps_c)), eng.h)
-        check(L_.bjx_chees_metric_init(eng.h, ptr(ms), n_ranks, options, ptr(imm)), eng.h)
-        # the update rewrites imm and re-installs it on the handle: the kernel's metric cache stays keyed on this tensor
-        eng._imm, eng._imm_key = imm, (imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device))
-        window_start = int(mass_matrix_window_fraction * num_steps)          # chees_adaptation.py:799
-        floor_on = bool(options & CHEES_LENGTH_FLOOR)
-        keys = bjx_random.split(rng_key.to(dev), num_steps)
-        for t in range(num_steps):
-            init_q = state.position
-            state, info = kernel(keys[t], state, logdensity_fn, eps_c, imm, steps_c)
-            in_window = t >= window_start
-            recompute = floor_on and in_window and t % LENGTH_FLOOR_RECOMPUTE_INTERVAL == 0
-            check(L_.bjx_chees_update_metric(eng.h, comm, n_ranks, options, ptr(st), ptr(ms), ptr(init_q),
-                                             ptr(info.proposal.position), ptr(info.proposal.momentum), ptr(state.position),
-                                             ptr(info.acceptance_rate), ptr(info.is_divergent.to(torch.uint8)),
-                                             float(optim.learning_rate), float(optim.b1), float(optim.b2),
-                                             float(target_acceptance_rate), float(decay_rate), int(max_leapfrog_steps),
-                                             int(in_window), int(recompute), ptr(eps_c), ptr(steps_c), ptr(hist), ptr(imm),
-                                             ptr(lam), ptr(eng_flag)), eng.h)
-        import ctypes as C_
-        out = (C_.c_float * 4)()
-        check(L_.bjx_chees_final_metric(eng.h, comm, n_ranks, options, ptr(st), ptr(ms), int(max_leapfrog_steps), ptr(imm),
-                                        out), eng.h)                 # the one host read of the warm-up
-        imm.add_(0.0)  # version bump: later users of imm re-derive mass_matrix_sqrt from the contents the device wrote
-        eng._imm_key = (imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device))
-        step, n_lf, clipped = float(out[0]), float(out[1]), bool(out[2])
-        jitter = lambda i: halton_sequence(i, max_bits) * jitter_amount + (1.0 - jitter_amount)
-        parameters = {
-            "step_size": step,
-            "inverse_mass_matrix": imm,
-            "next_random_arg_fn": lambda i: i + 1,
-            "integration_steps_fn": lambda i, n: int(math.ceil(jitter(i) * n)),
-            "integration_steps_params": (n_lf,),
-        }
-        last = dynamic_hmc.DynamicHMCState(state.position, state.logdensity, state.logdensity_grad, num_steps)
-        return AdaptationResults(last, parameters), ChEESMetricInfo(hist.cpu(), lam.cpu(), eng_flag.cpu().bool(), clipped)
 
     return AdaptationAlgorithm(run)

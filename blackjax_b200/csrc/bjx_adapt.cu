@@ -434,35 +434,12 @@ __device__ __forceinline__ void mm_fold_diag(int D, int d, int nblk, int nbl, si
   ms[kMmHdr + D + d] = ms[kMmHdr + D + d] + m2 + delta * delta * fc;
 }
 
-// merge the pass-1 blocks in global order: proposal mean (weighted), initial mean (nanmean), harmonic-mean sums
-__global__ void k_chees_means(int D, int nblk, const float* __restrict__ blocks, float* __restrict__ st) {
-  const size_t S = 3 + 3 * (size_t)D;
-  float* pm = st + kChHdr;
-  float* qm = pm + D;
-  float sw = 0.f;
-  for (int b = 0; b < nblk; ++b) sw += blocks[b * S + 2];
-  for (int d = threadIdx.x; d < D; d += blockDim.x) {
-    float a = 0.f, q = 0.f, n = 0.f;
-    for (int b = 0; b < nblk; ++b) {
-      a += blocks[b * S + 3 + d];
-      q += blocks[b * S + 3 + D + d];
-      n += blocks[b * S + 3 + 2 * D + d];
-    }
-    pm[d] = a / (sw + 1e-20f);
-    qm[d] = q / n;
-  }
-  if (threadIdx.x == 0) {
-    float h = 0.f, n = 0.f;
-    for (int b = 0; b < nblk; ++b) { h += blocks[b * S]; n += blocks[b * S + 1]; }
-    st[CH_HM_SUM] = h;
-    st[CH_HM_N] = n;
-  }
-}
-// k_chees_means for the diagonal-metric mode: the same sums in the same order over a rank-major payload of R floats per
-// rank, [nbl pass-1 blocks | nbl k_block_stats blocks of the new positions]; with in_window the latter are folded into the
-// diagonal accumulator of `ms`
-__global__ void k_chees_means_metric(int D, int nblk, const float* __restrict__ blocks, float* __restrict__ st, int nbl, size_t R,
-                                     float* __restrict__ ms, int in_window) {
+// merge the pass-1 blocks in global order: proposal mean (weighted), initial mean (nanmean), harmonic-mean sums.  The
+// payload is rank-major, R floats per rank, starting with the rank's nbl pass-1 blocks (the identity metric: R = nbl * S,
+// so block b is at b * S).  The diagonal-metric payload follows them with the rank's nbl k_block_stats blocks of the new
+// positions; with in_window these are folded into the diagonal accumulator of `ms`.
+__global__ void k_chees_means(int D, int nblk, const float* __restrict__ blocks, float* __restrict__ st, int nbl, size_t R,
+                              float* __restrict__ ms, int in_window) {
   const size_t S = 3 + 3 * (size_t)D;
   auto blk = [&](int b) { return blocks + (size_t)(b / nbl) * R + (size_t)(b % nbl) * S; };
   float* pm = st + kChHdr;
@@ -551,13 +528,12 @@ __global__ void k_chees_pass2(int C, const float* __restrict__ num, const float*
 }
 
 // the scalar update (chees_adaptation.py:341-360,470-511) and the next transition's step count.
-// kMetric: the next transition consumes min(max(T, floor), max_leapfrog * eps) with floor = (pi/2) sqrt(lambda_max) once the
-// diagonal estimate is engaged (_apply_length_floor, :192-236); T itself, the optimiser's state, is never floored.
-template <bool kMetric = false>
+// With a metric state `ms` whose length floor is on, the next transition consumes min(max(T, floor), max_leapfrog * eps)
+// with floor = (pi/2) sqrt(lambda_max) once the diagonal estimate is engaged (_apply_length_floor, :192-236); T itself, the
+// optimiser's state, is never floored.  lam_hist and eng_hist need `ms`.
 __global__ void k_chees_finish(int nblk, const float* __restrict__ blocks2, float* __restrict__ st, float lr, float b1, float b2,
                                float target, float decay, float max_leapfrog, float* __restrict__ hist,
-                               const float* __restrict__ ms = nullptr, float* __restrict__ lam_hist = nullptr,
-                               float* __restrict__ eng_hist = nullptr) {
+                               const float* __restrict__ ms, float* __restrict__ lam_hist, float* __restrict__ eng_hist) {
   if (threadIdx.x != 0) return;
   const int max_bits = (int)st[CH_MAX_BITS];
   const float jam = st[CH_JITTER_AMOUNT];
@@ -610,22 +586,16 @@ __global__ void k_chees_finish(int nblk, const float* __restrict__ blocks2, floa
   st[CH_GRAD] = grad;
   // next transition: ceil(jitter(i + 1) * T / eps) leapfrog steps (integration_steps_fn :775-779)
   const float jn = halton_f(rga + 1, max_bits) * jam + (1.f - jam);
-  if constexpr (kMetric) {
-    float consumed = newT;
-    if (ms[MM_FLOOR] != 0.f) {
-      const float floor_v = ms[MM_ENGAGED] != 0.f ? 1.57079637f * sqrtf(ms[MM_LAMBDA]) : 0.f;
-      consumed = fminf(fmaxf(newT, floor_v), max_leapfrog * eps);
-    }
-    st[CH_L] = ceilf(jn * (consumed / eps));
-  } else {
-    st[CH_L] = ceilf(jn * (newT / eps));
+  float consumed = newT;
+  if (ms && ms[MM_FLOOR] != 0.f) {
+    const float floor_v = ms[MM_ENGAGED] != 0.f ? 1.57079637f * sqrtf(ms[MM_LAMBDA]) : 0.f;
+    consumed = fminf(fmaxf(newT, floor_v), max_leapfrog * eps);
   }
+  st[CH_L] = ceilf(jn * (consumed / eps));
   const int t = (int)st[CH_T_IDX];
   if (hist) { hist[4 * t] = eps; hist[4 * t + 1] = newT; hist[4 * t + 2] = st[CH_L]; hist[4 * t + 3] = grad; }
-  if constexpr (kMetric) {
-    if (lam_hist) lam_hist[t] = ms[MM_LAMBDA];
-    if (eng_hist) eng_hist[t] = ms[MM_ENGAGED];
-  }
+  if (lam_hist) lam_hist[t] = ms[MM_LAMBDA];
+  if (eng_hist) eng_hist[t] = ms[MM_ENGAGED];
   st[CH_T_IDX] = (float)(t + 1);
 }
 __global__ void k_chees_init(float* st, float eps0, int max_bits, float jitter_amount) {
@@ -841,27 +811,226 @@ __global__ void k_mm_init(int D, float* __restrict__ ms, float c_global, float t
   }
 }
 
-// The block covariance accumulators on their own, for MEADS-LRD (bjx_meads.cu); the same kernels and block order as above.
+// The launchers of the block statistics and the block covariance accumulators, shared by ChEES and MEADS-LRD (bjx_meads.cu).
 int cov_stat_blocks(int C) { return n_stat_blocks(C); }
 size_t cov_block_floats(int D) { return 2 + (size_t)D + (size_t)D * D; }
-void launch_cov_fold(int C, int D, const float* q, float* stats, float* cov, cudaStream_t s) {
+void launch_block_stats(int C, int D, const float* x, const float* acc, float* out, cudaStream_t s) {
+  k_block_stats<<<dim3((D + 31) / 32, n_stat_blocks(C)), dim3(32, 8), 0, s>>>(C, D, x, acc, out);
+}
+void launch_cov_fold(int C, int D, const float* q, const float* stats, float* cov, cudaStream_t s) {
   const int nb = n_stat_blocks(C), tiles = (D + kSyT - 1) / kSyT;
   const size_t sstride = 2 + 2 * (size_t)D;
-  // k_block_stats also sums an acceptance array over each block; q stands in for it (that sum is not read here)
-  k_block_stats<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, q, q, stats);
   k_cov_syrk<<<dim3(tiles * (tiles + 1) / 2, nb), 256, 0, s>>>(C, D, q, stats, sstride, cov, cov_block_floats(D));
   k_cov_mean_update<<<nb, 256, 0, s>>>(C, D, stats, sstride, cov, cov_block_floats(D));
 }
-void launch_cov_merge(int C, int D, const float* cov, float* out, float* count_mean, cudaStream_t s) {
-  k_cov_merge_whiten<<<dim3((D + 255) / 256, D), 256, 0, s>>>(D, n_stat_blocks(C), cov, cov_block_floats(D), nullptr, out,
-                                                             count_mean);
+void launch_cov_merge(int nblk, int D, const float* cov, const float* imm, float* out, float* count_mean, cudaStream_t s) {
+  k_cov_merge_whiten<<<dim3((D + 255) / 256, D), 256, 0, s>>>(D, nblk, cov, cov_block_floats(D), imm, out, count_mean);
 }
 }  // namespace bjx
 
+// =====================================================================================================================
+// ChEES with mass_matrix_estimation="diagonal" (chees_adaptation.py:61-237,797-1001).  The metric state holds the diagonal
+// accumulator, the power-iteration vectors, this step's payload for the first all-gather (the pass-1 blocks followed by the
+// k_block_stats blocks of the new positions, so an ordinary step adds no collective) and, with the length floor, the
+// per-block covariance accumulators and the whitened matrix of the last recompute.  Only recompute steps (every 32
+// in-window steps, and the final parameters) move D x D data between GPUs: the block accumulators are all-gathered and
+// merged in global block order on every rank (DESIGN.md section 7).
+// =====================================================================================================================
+namespace {
+// The ChEES state of both modes: header, proposal mean[D], initial mean[D], the per-chain w, num and den [C], the pass-1
+// blocks of this rank and of all ranks (the identity metric's payload; the diagonal metric gathers its own), and the
+// pass-2 blocks (sum num, sum den) of this rank and of all ranks.
+struct ChLayout {
+  int nb;
+  size_t S1;                                                     // pass-1 record stride
+  size_t w, num, den, loc1, gat1, loc2, gat2, total;
+};
+ChLayout ch_layout(int C, int D, int n_ranks) {
+  ChLayout L{};
+  L.nb = n_stat_blocks(C);
+  L.S1 = 3 + 3 * (size_t)D;
+  size_t o = kChHdr + 2 * (size_t)D;
+  L.w = o; o += C;
+  L.num = o; o += C;
+  L.den = o; o += C;
+  L.loc1 = o; o += (size_t)L.nb * L.S1;
+  L.gat1 = o; o += (size_t)L.nb * L.S1 * n_ranks;
+  L.loc2 = o; o += (size_t)L.nb * 2;
+  L.gat2 = o; o += (size_t)L.nb * 2 * n_ranks;
+  L.total = o;
+  return L;
+}
+
+struct MmLayout {
+  int nb;
+  size_t S1, Sm, R, Sc;                                          // record strides; R = payload floats per rank
+  size_t eig, u0, u1, pay_loc, pay_stats, W, cov_loc, pay_gat, cov_gat, total;
+};
+MmLayout mm_layout(int C, int D, int n_ranks, int options) {
+  MmLayout L{};
+  const size_t d = (size_t)D;
+  const bool fl = options & BJX_CHEES_LENGTH_FLOOR;
+  L.nb = n_stat_blocks(C);
+  L.S1 = 3 + 3 * d;
+  L.Sm = 2 + 2 * d;
+  L.R = (size_t)L.nb * (L.S1 + L.Sm);
+  L.Sc = cov_block_floats(D);
+  size_t o = kMmHdr + 2 * d;                                     // header, accumulator mean[D], m2[D]
+  L.eig = o; o += d;
+  L.u0 = o; o += d;
+  L.u1 = o; o += d;
+  L.pay_loc = o;                                                 // payload: pass-1 blocks, then the k_block_stats blocks
+  L.pay_stats = o + (size_t)L.nb * L.S1; o += L.R;
+  L.W = o; o += fl ? d * d : 0;
+  L.cov_loc = o; o += fl ? (size_t)L.nb * L.Sc : 0;
+  L.pay_gat = o; o += n_ranks > 1 ? L.R * n_ranks : 0;
+  L.cov_gat = o; o += (fl && n_ranks > 1) ? (size_t)L.nb * L.Sc * n_ranks : 0;
+  L.total = o;
+  return L;
+}
+
+// merged block accumulators -> W (whitened by imm, or the plain covariance with imm = NULL); block order is global
+int mm_cov_merge(bjx_handle_t h, void* comm, int n_ranks, const MmLayout& L, float* ms, const float* imm, float* W,
+                 float* mean_out) {
+  const float* cov = ms + L.cov_loc;
+  if (n_ranks > 1) {
+    int rc = bjx_allgather_stats(h, comm, ms + L.cov_loc, (int64_t)(L.nb * L.Sc), ms + L.cov_gat);
+    if (rc) return rc;
+    cov = ms + L.cov_gat;
+  }
+  launch_cov_merge(L.nb * n_ranks, h->cfg.dim, cov, imm, W, mean_out, h->stream);
+  BJX_CHECK_LAUNCH("k_cov_merge_whiten");
+  return 0;
+}
+
+// _recompute_eig_state: whiten by imm, `iters` power iterations warm-started from the stored eigenvector, lambda_max
+int mm_recompute(bjx_handle_t h, void* comm, int n_ranks, const MmLayout& L, float* ms, const float* imm, int iters) {
+  const int D = h->cfg.dim;
+  int rc = mm_cov_merge(h, comm, n_ranks, L, ms, imm, ms + L.W, nullptr);
+  if (rc) return rc;
+  const float* W = ms + L.W;
+  float* u[2] = {ms + L.u0, ms + L.u1};
+  const int g = (D + 7) / 8;
+  k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, ms + L.eig, 0, nullptr, u[0]);
+  for (int k = 1; k < iters; ++k) k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, u[(k - 1) & 1], 1, nullptr, u[k & 1]);
+  k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, u[(iters - 1) & 1], 1, ms + L.eig, u[iters & 1]);
+  k_pow_rayleigh<<<1, 256, 0, h->stream>>>(D, ms + L.eig, u[iters & 1], ms);
+  BJX_CHECK_LAUNCH("k_pow_iter");
+  return 0;
+}
+
+constexpr int kFloorIters = 5, kFloorFinalIters = 20;  // chees_adaptation.py:121-122 (the 32-step cadence is the caller's)
+
+// One warm-up step of either mode.  The identity metric has no metric state (ms = NULL, options = 0, no window): its
+// pass-1 payload is the state's.  The diagonal metric gathers the metric state's payload; its in-window steps fold the new
+// positions into the diagonal accumulator (and, with the length floor, the covariance accumulators) and rewrite imm.
+int chees_step(bjx_handle_t h, void* comm, int n_ranks, int options, float* state, float* ms, const float* init_q,
+               const float* prop_q, const float* prop_p, const float* new_q, const float* acc, const uint8_t* is_div,
+               float lr, float b1, float b2, float target, float decay, int max_lf, int in_window, int recompute,
+               float* eps_c, int32_t* steps_c, float* hist, float* imm, float* lam_hist, float* eng_hist) {
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  const ChLayout L = ch_layout(C, D, n_ranks);
+  const int nb = L.nb;
+  MmLayout M{};
+  float* pay = state + L.loc1;
+  float* pay_gat = state + L.gat1;
+  size_t R = (size_t)nb * L.S1;
+  if (ms) {
+    M = mm_layout(C, D, n_ranks, options);
+    pay = ms + M.pay_loc;
+    pay_gat = ms + M.pay_gat;
+    R = M.R;
+  }
+  float* w = state + L.w;
+  float* num = state + L.num;
+  float* den = state + L.den;
+  cudaStream_t s = h->stream;
+  k_chees_w<<<(C + 7) / 8, 256, 0, s>>>(C, D, prop_q, acc, is_div, w);
+  k_chees_pass1<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, prop_q, init_q, acc, is_div, w, pay);
+  BJX_CHECK_LAUNCH("k_chees_pass1");
+  if (in_window) {
+    launch_block_stats(C, D, new_q, acc, ms + M.pay_stats, s);
+    BJX_CHECK_LAUNCH("k_block_stats");
+  }
+  const float* m1 = pay;
+  if (n_ranks > 1) {
+    int rc = bjx_allgather_stats(h, comm, pay, (int64_t)R, pay_gat);
+    if (rc) return rc;
+    m1 = pay_gat;
+  }
+  k_chees_means<<<1, 512, 0, s>>>(D, nb * n_ranks, m1, state, nb, R, ms, in_window);
+  if (options & BJX_CHEES_WHITEN)  // the criterion of this step uses the metric of this step's transition
+    k_chees_dots<true><<<(C + 7) / 8, 256, 0, s>>>(C, D, prop_q, prop_p, init_q, acc, is_div, state, num, den, imm);
+  else
+    k_chees_dots<<<(C + 7) / 8, 256, 0, s>>>(C, D, prop_q, prop_p, init_q, acc, is_div, state, num, den);
+  k_chees_pass2<<<nb, 256, 0, s>>>(C, num, den, state + L.loc2);
+  BJX_CHECK_LAUNCH("k_chees_pass2");
+  const float* m2 = state + L.loc2;
+  if (n_ranks > 1) {
+    int rc = bjx_allgather_stats(h, comm, state + L.loc2, (int64_t)(nb * 2), state + L.gat2);
+    if (rc) return rc;
+    m2 = state + L.gat2;
+  }
+  if (in_window && (options & BJX_CHEES_LENGTH_FLOOR)) {
+    launch_cov_fold(C, D, new_q, ms + M.pay_stats, ms + M.cov_loc, s);
+    BJX_CHECK_LAUNCH("k_cov_syrk");
+    if (recompute) {  // against the metric this step's transition used, before this step's fold engages (:898-903)
+      int rc = mm_recompute(h, comm, n_ranks, M, ms, imm, kFloorIters);
+      if (rc) return rc;
+    }
+  }
+  if (in_window) {
+    k_mm_imm<<<1, 1024, 0, s>>>(D, ms, imm);
+    BJX_CHECK_LAUNCH("k_mm_imm");
+  }
+  k_chees_finish<<<1, 32, 0, s>>>(nb * n_ranks, m2, state, lr, b1, b2, target, decay, (float)max_lf, hist, ms, lam_hist,
+                                  eng_hist);
+  k_fill_from<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_EPS, eps_c);
+  k_fill_steps<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_L, steps_c);
+  BJX_CHECK_LAUNCH("k_chees_finish");
+  if (in_window) return bjx_set_metric(h, BJX_METRIC_DIAG, imm);  // mass_matrix_sqrt of the new estimate, on the stream
+  return 0;
+}
+
+// Final parameters (:958-1001), on the host: out[0] = exp(log eps_ma), out[1] = exp(log T_ma - log eps_ma).  With the
+// length floor, 20 power iterations against the final metric (:971-978) come first and the floor is re-applied to
+// exp(log T_ma), divided by exp(log eps_ma).  With a metric state, out[2] = floor clipped by the cap, out[3] = lambda_max.
+int chees_final(bjx_handle_t h, void* comm, int n_ranks, int options, const float* state, float* ms, int max_lf,
+                const float* imm, float* out) {
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  const bool floor_on = options & BJX_CHEES_LENGTH_FLOOR;
+  if (floor_on) {
+    int rc = mm_recompute(h, comm, n_ranks, mm_layout(h->cfg.n_chains, h->cfg.dim, n_ranks, options), ms, imm,
+                          kFloorFinalIters);
+    if (rc) return rc;
+  }
+  float hst[kChHdr], hdr[kMmHdr];
+  BJX_CUDA(cudaMemcpyAsync(hst, state, sizeof(hst), cudaMemcpyDeviceToHost, h->stream));
+  if (ms) BJX_CUDA(cudaMemcpyAsync(hdr, ms, sizeof(hdr), cudaMemcpyDeviceToHost, h->stream));
+  BJX_CUDA(cudaStreamSynchronize(h->stream));
+  const float eps = expf(hst[CH_LOG_EPS_MA]);
+  float n_lf = expf(hst[CH_LOG_T_MA] - hst[CH_LOG_EPS_MA]), clipped = 0.f;
+  if (floor_on) {
+    const bool engaged = hdr[MM_ENGAGED] != 0.f;
+    const float floor_v = engaged ? 1.57079637f * sqrtf(hdr[MM_LAMBDA]) : 0.f;
+    const float cap = (float)max_lf * eps;
+    n_lf = fminf(fmaxf(expf(hst[CH_LOG_T_MA]), floor_v), cap) / eps;
+    clipped = (engaged && floor_v > cap) ? 1.f : 0.f;
+  }
+  out[0] = eps;
+  out[1] = n_lf;
+  if (ms) {
+    out[2] = clipped;
+    out[3] = hdr[MM_LAMBDA];
+  }
+  return 0;
+}
+}  // namespace
+
 extern "C" int64_t bjx_chees_state_floats(int32_t n_chains_local, int32_t dim, int32_t n_ranks) {
   if (n_chains_local <= 0 || dim <= 0 || n_ranks <= 0) return 0;
-  const int64_t nb = n_stat_blocks(n_chains_local), D = dim;
-  return kChHdr + 2 * D + 3 * (int64_t)n_chains_local + nb * (3 + 3 * D) * (1 + n_ranks) + nb * 2 * (1 + n_ranks);
+  return (int64_t)ch_layout(n_chains_local, dim, n_ranks).total;
 }
 
 extern "C" int bjx_chees_init(bjx_handle_t h, float* state, float step_size, int32_t max_bits, float jitter_amount,
@@ -887,137 +1056,15 @@ extern "C" int bjx_chees_update(bjx_handle_t h, void* nccl_comm, int32_t n_ranks
       !step_size_chain || !steps_chain)
     return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
-  BJX_CUDA(cudaSetDevice(h->cfg.device));
-  const int C = h->cfg.n_chains, D = h->cfg.dim;
-  const int nb = n_stat_blocks(C);
-  const size_t S1 = 3 + 3 * (size_t)D;
-  float* w = state + kChHdr + 2 * (size_t)D;
-  float* num = w + C;
-  float* den = num + C;
-  float* loc1 = den + C;
-  float* gat1 = loc1 + (size_t)nb * S1;
-  float* loc2 = gat1 + (size_t)nb * S1 * n_ranks;
-  float* gat2 = loc2 + (size_t)nb * 2;
-  cudaStream_t s = h->stream;
-  k_chees_w<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, acceptance_rate, is_divergent, w);
-  k_chees_pass1<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, proposal_position, initial_position, acceptance_rate,
-                                                              is_divergent, w, loc1);
-  BJX_CHECK_LAUNCH("k_chees_pass1");
-  const float* m1 = loc1;
-  if (n_ranks > 1) {
-    int rc = bjx_allgather_stats(h, nccl_comm, loc1, (int64_t)(nb * S1), gat1);
-    if (rc) return rc;
-    m1 = gat1;
-  }
-  k_chees_means<<<1, 512, 0, s>>>(D, nb * n_ranks, m1, state);
-  k_chees_dots<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, proposal_momentum, initial_position, acceptance_rate,
-                                          is_divergent, state, num, den);
-  k_chees_pass2<<<nb, 256, 0, s>>>(C, num, den, loc2);
-  BJX_CHECK_LAUNCH("k_chees_pass2");
-  const float* m2 = loc2;
-  if (n_ranks > 1) {
-    int rc = bjx_allgather_stats(h, nccl_comm, loc2, (int64_t)(nb * 2), gat2);
-    if (rc) return rc;
-    m2 = gat2;
-  }
-  k_chees_finish<<<1, 32, 0, s>>>(nb * n_ranks, m2, state, learning_rate, b1, b2, target_acceptance, decay_rate,
-                                  (float)max_leapfrog_steps, history);
-  k_fill_from<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_EPS, step_size_chain);
-  k_fill_steps<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_L, steps_chain);
-  BJX_CHECK_LAUNCH("k_chees_finish");
-  return 0;
+  return chees_step(h, nccl_comm, n_ranks, 0, state, nullptr, initial_position, proposal_position, proposal_momentum, nullptr,
+                    acceptance_rate, is_divergent, learning_rate, b1, b2, target_acceptance, decay_rate, max_leapfrog_steps,
+                    0, 0, step_size_chain, steps_chain, history, nullptr, nullptr, nullptr);
 }
 
 extern "C" int bjx_chees_final(bjx_handle_t h, const float* state, float* out2) {
   if (!h || !state || !out2) return bjx_fail(h, BJX_E_INVALID, "null argument");
-  BJX_CUDA(cudaSetDevice(h->cfg.device));
-  float hst[kChHdr];
-  BJX_CUDA(cudaMemcpyAsync(hst, state, sizeof(hst), cudaMemcpyDeviceToHost, h->stream));
-  BJX_CUDA(cudaStreamSynchronize(h->stream));
-  out2[0] = expf(hst[CH_LOG_EPS_MA]);                       // step_size
-  out2[1] = expf(hst[CH_LOG_T_MA] - hst[CH_LOG_EPS_MA]);    // num_leapfrog_steps (integration_steps_params)
-  return 0;
+  return chees_final(h, nullptr, 1, 0, state, nullptr, 0, nullptr, out2);
 }
-
-// =====================================================================================================================
-// ChEES with mass_matrix_estimation="diagonal" (chees_adaptation.py:61-237,797-1001).  The metric state holds the diagonal
-// accumulator, the power-iteration vectors, this step's payload for the first all-gather (the pass-1 blocks followed by the
-// k_block_stats blocks of the new positions, so an ordinary step adds no collective) and, with the length floor, the
-// per-block covariance accumulators and the whitened matrix of the last recompute.  Only recompute steps (every 32
-// in-window steps, and the final parameters) move D x D data between GPUs: the block accumulators are all-gathered and
-// merged in global block order on every rank (DESIGN.md section 7).
-// =====================================================================================================================
-namespace {
-struct MmLayout {
-  int nb;
-  size_t S1, Sm, R, Sc;                                          // record strides; R = payload floats per rank
-  size_t eig, u0, u1, pay_loc, W, cov_loc, pay_gat, cov_gat, total;
-};
-MmLayout mm_layout(int C, int D, int n_ranks, int options) {
-  MmLayout L{};
-  const size_t d = (size_t)D;
-  const bool fl = options & BJX_CHEES_LENGTH_FLOOR;
-  L.nb = n_stat_blocks(C);
-  L.S1 = 3 + 3 * d;
-  L.Sm = 2 + 2 * d;
-  L.R = (size_t)L.nb * (L.S1 + L.Sm);
-  L.Sc = 2 + d + d * d;
-  size_t o = kMmHdr + 2 * d;                                     // header, accumulator mean[D], m2[D]
-  L.eig = o; o += d;
-  L.u0 = o; o += d;
-  L.u1 = o; o += d;
-  L.pay_loc = o; o += L.R;
-  L.W = o; o += fl ? d * d : 0;
-  L.cov_loc = o; o += fl ? (size_t)L.nb * L.Sc : 0;
-  L.pay_gat = o; o += n_ranks > 1 ? L.R * n_ranks : 0;
-  L.cov_gat = o; o += (fl && n_ranks > 1) ? (size_t)L.nb * L.Sc * n_ranks : 0;
-  L.total = o;
-  return L;
-}
-
-// fold new positions q [C, D] into the block covariance accumulators; their k_block_stats records are at stats
-int cov_fold(bjx_handle_t h, const MmLayout& L, float* ms, const float* q, const float* stats) {
-  const int C = h->cfg.n_chains, D = h->cfg.dim;
-  const int tiles = (D + kSyT - 1) / kSyT;
-  k_cov_syrk<<<dim3(tiles * (tiles + 1) / 2, L.nb), 256, 0, h->stream>>>(C, D, q, stats, L.Sm, ms + L.cov_loc, L.Sc);
-  BJX_CHECK_LAUNCH("k_cov_syrk");
-  k_cov_mean_update<<<L.nb, 256, 0, h->stream>>>(C, D, stats, L.Sm, ms + L.cov_loc, L.Sc);
-  BJX_CHECK_LAUNCH("k_cov_mean_update");
-  return 0;
-}
-
-// merged block accumulators -> W (whitened by imm, or the plain covariance with imm = NULL); block order is global
-int cov_merge(bjx_handle_t h, void* comm, int n_ranks, const MmLayout& L, float* ms, const float* imm, float* W, float* mean_out) {
-  const int D = h->cfg.dim;
-  const float* cov = ms + L.cov_loc;
-  if (n_ranks > 1) {
-    int rc = bjx_allgather_stats(h, comm, ms + L.cov_loc, (int64_t)(L.nb * L.Sc), ms + L.cov_gat);
-    if (rc) return rc;
-    cov = ms + L.cov_gat;
-  }
-  k_cov_merge_whiten<<<dim3((D + 255) / 256, D), 256, 0, h->stream>>>(D, L.nb * n_ranks, cov, L.Sc, imm, W, mean_out);
-  BJX_CHECK_LAUNCH("k_cov_merge_whiten");
-  return 0;
-}
-
-// _recompute_eig_state: whiten by imm, `iters` power iterations warm-started from the stored eigenvector, lambda_max
-int mm_recompute(bjx_handle_t h, void* comm, int n_ranks, const MmLayout& L, float* ms, const float* imm, int iters) {
-  const int D = h->cfg.dim;
-  int rc = cov_merge(h, comm, n_ranks, L, ms, imm, ms + L.W, nullptr);
-  if (rc) return rc;
-  const float* W = ms + L.W;
-  float* u[2] = {ms + L.u0, ms + L.u1};
-  const int g = (D + 7) / 8;
-  k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, ms + L.eig, 0, nullptr, u[0]);
-  for (int k = 1; k < iters; ++k) k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, u[(k - 1) & 1], 1, nullptr, u[k & 1]);
-  k_pow_iter<<<g, 256, 0, h->stream>>>(D, W, u[(iters - 1) & 1], 1, ms + L.eig, u[iters & 1]);
-  k_pow_rayleigh<<<1, 256, 0, h->stream>>>(D, ms + L.eig, u[iters & 1], ms);
-  BJX_CHECK_LAUNCH("k_pow_iter");
-  return 0;
-}
-
-constexpr int kFloorIters = 5, kFloorFinalIters = 20;  // chees_adaptation.py:121-122 (the 32-step cadence is the caller's)
-}  // namespace
 
 extern "C" int64_t bjx_chees_metric_state_floats(int32_t n_chains_local, int32_t dim, int32_t n_ranks, int32_t options) {
   if (n_chains_local <= 0 || dim <= 0 || dim > 1024 || n_ranks <= 0) return 0;
@@ -1050,104 +1097,21 @@ extern "C" int bjx_chees_update_metric(bjx_handle_t h, void* nccl_comm, int32_t 
       !acceptance_rate || !is_divergent || !step_size_chain || !steps_chain || !imm)
     return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
-  const bool floor_on = options & BJX_CHEES_LENGTH_FLOOR;
-  if (recompute && !(in_window && floor_on))
+  if (recompute && !(in_window && (options & BJX_CHEES_LENGTH_FLOOR)))
     return bjx_fail(h, BJX_E_INVALID, "recompute needs an in-window step and the length floor");
-  BJX_CUDA(cudaSetDevice(h->cfg.device));
-  const int C = h->cfg.n_chains, D = h->cfg.dim;
-  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
-  const MmLayout L = mm_layout(C, D, n_ranks, options);
-  const int nb = L.nb;
-  float* ms = metric_state;
-  float* w = state + kChHdr + 2 * (size_t)D;
-  float* num = w + C;
-  float* den = num + C;
-  float* loc2 = den + C + (size_t)nb * L.S1 * (1 + n_ranks);  // the pass-2 regions of the identity-metric layout
-  float* gat2 = loc2 + (size_t)nb * 2;
-  float* loc1 = ms + L.pay_loc;
-  float* locm = loc1 + (size_t)nb * L.S1;                     // k_block_stats records of the new positions
-  cudaStream_t s = h->stream;
-  k_chees_w<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, acceptance_rate, is_divergent, w);
-  k_chees_pass1<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, proposal_position, initial_position, acceptance_rate,
-                                                              is_divergent, w, loc1);
-  BJX_CHECK_LAUNCH("k_chees_pass1");
-  if (in_window) {
-    k_block_stats<<<dim3((D + 31) / 32, nb), dim3(32, 8), 0, s>>>(C, D, new_position, acceptance_rate, locm);
-    BJX_CHECK_LAUNCH("k_block_stats");
-  }
-  const float* m1 = loc1;
-  if (n_ranks > 1) {
-    int rc = bjx_allgather_stats(h, nccl_comm, loc1, (int64_t)L.R, ms + L.pay_gat);
-    if (rc) return rc;
-    m1 = ms + L.pay_gat;
-  }
-  k_chees_means_metric<<<1, 512, 0, s>>>(D, nb * n_ranks, m1, state, nb, L.R, ms, in_window);
-  if (options & BJX_CHEES_WHITEN)  // the criterion of this step uses the metric of this step's transition
-    k_chees_dots<true><<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, proposal_momentum, initial_position, acceptance_rate,
-                                                   is_divergent, state, num, den, imm);
-  else
-    k_chees_dots<<<(C + 7) / 8, 256, 0, s>>>(C, D, proposal_position, proposal_momentum, initial_position, acceptance_rate,
-                                             is_divergent, state, num, den);
-  k_chees_pass2<<<nb, 256, 0, s>>>(C, num, den, loc2);
-  BJX_CHECK_LAUNCH("k_chees_pass2");
-  const float* m2 = loc2;
-  if (n_ranks > 1) {
-    int rc = bjx_allgather_stats(h, nccl_comm, loc2, (int64_t)(nb * 2), gat2);
-    if (rc) return rc;
-    m2 = gat2;
-  }
-  if (in_window && floor_on) {
-    int rc = cov_fold(h, L, ms, new_position, locm);
-    if (rc) return rc;
-    if (recompute) {  // against the metric this step's transition used, before this step's fold engages (:898-903)
-      rc = mm_recompute(h, nccl_comm, n_ranks, L, ms, imm, kFloorIters);
-      if (rc) return rc;
-    }
-  }
-  if (in_window) {
-    k_mm_imm<<<1, 1024, 0, s>>>(D, ms, imm);
-    BJX_CHECK_LAUNCH("k_mm_imm");
-  }
-  k_chees_finish<true><<<1, 32, 0, s>>>(nb * n_ranks, m2, state, learning_rate, b1, b2, target_acceptance, decay_rate,
-                                        (float)max_leapfrog_steps, history, ms, lambda_history, engaged_history);
-  k_fill_from<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_EPS, step_size_chain);
-  k_fill_steps<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_L, steps_chain);
-  BJX_CHECK_LAUNCH("k_chees_finish");
-  if (in_window) return bjx_set_metric(h, BJX_METRIC_DIAG, imm);  // mass_matrix_sqrt of the new estimate, on the stream
-  return 0;
+  if (h->cfg.dim > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  return chees_step(h, nccl_comm, n_ranks, options, state, metric_state, initial_position, proposal_position,
+                    proposal_momentum, new_position, acceptance_rate, is_divergent, learning_rate, b1, b2, target_acceptance,
+                    decay_rate, max_leapfrog_steps, in_window, recompute, step_size_chain, steps_chain, history, imm,
+                    lambda_history, engaged_history);
 }
 
 extern "C" int bjx_chees_final_metric(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, const float* state,
                                       float* metric_state, int32_t max_leapfrog_steps, const float* imm, float* out4_host) {
   if (!h || !state || !metric_state || !imm || !out4_host) return bjx_fail(h, BJX_E_INVALID, "null argument");
   if (n_ranks < 1 || (n_ranks > 1 && !nccl_comm)) return bjx_fail(h, BJX_E_INVALID, "n_ranks > 1 needs a communicator");
-  BJX_CUDA(cudaSetDevice(h->cfg.device));
-  const int C = h->cfg.n_chains, D = h->cfg.dim;
-  if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
-  const MmLayout L = mm_layout(C, D, n_ranks, options);
-  if (options & BJX_CHEES_LENGTH_FLOOR) {  // 20 power iterations against the final metric (:971-978)
-    int rc = mm_recompute(h, nccl_comm, n_ranks, L, metric_state, imm, kFloorFinalIters);
-    if (rc) return rc;
-  }
-  float hst[kChHdr], hdr[kMmHdr];
-  BJX_CUDA(cudaMemcpyAsync(hst, state, sizeof(hst), cudaMemcpyDeviceToHost, h->stream));
-  BJX_CUDA(cudaMemcpyAsync(hdr, metric_state, sizeof(hdr), cudaMemcpyDeviceToHost, h->stream));
-  BJX_CUDA(cudaStreamSynchronize(h->stream));
-  // final parameters (:958-1001), on the host as bjx_chees_final forms them
-  const float eps = expf(hst[CH_LOG_EPS_MA]);
-  float n_lf = expf(hst[CH_LOG_T_MA] - hst[CH_LOG_EPS_MA]), clipped = 0.f;
-  if (options & BJX_CHEES_LENGTH_FLOOR) {  // floor re-applied to exp(log T_ma), divided by exp(log eps_ma)
-    const bool engaged = hdr[MM_ENGAGED] != 0.f;
-    const float floor_v = engaged ? 1.57079637f * sqrtf(hdr[MM_LAMBDA]) : 0.f;
-    const float cap = (float)max_leapfrog_steps * eps;
-    n_lf = fminf(fmaxf(expf(hst[CH_LOG_T_MA]), floor_v), cap) / eps;
-    clipped = (engaged && floor_v > cap) ? 1.f : 0.f;
-  }
-  out4_host[0] = eps;
-  out4_host[1] = n_lf;
-  out4_host[2] = clipped;
-  out4_host[3] = hdr[MM_LAMBDA];
-  return 0;
+  if (h->cfg.dim > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
+  return chees_final(h, nccl_comm, n_ranks, options, state, metric_state, max_leapfrog_steps, imm, out4_host);
 }
 
 extern "C" int bjx_chees_metric_fold_covariance(bjx_handle_t h, int32_t options, float* metric_state, const float* q) {
@@ -1157,11 +1121,12 @@ extern "C" int bjx_chees_metric_fold_covariance(bjx_handle_t h, int32_t options,
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
   const MmLayout L = mm_layout(C, D, 1, options);
-  float* locm = metric_state + L.pay_loc + (size_t)L.nb * L.S1;
   // k_block_stats also sums an acceptance array over each block; q stands in for it (that sum is not read here)
-  k_block_stats<<<dim3((D + 31) / 32, L.nb), dim3(32, 8), 0, h->stream>>>(C, D, q, q, locm);
+  launch_block_stats(C, D, q, q, metric_state + L.pay_stats, h->stream);
   BJX_CHECK_LAUNCH("k_block_stats");
-  return cov_fold(h, L, metric_state, q, locm);
+  launch_cov_fold(C, D, q, metric_state + L.pay_stats, metric_state + L.cov_loc, h->stream);
+  BJX_CHECK_LAUNCH("k_cov_syrk");
+  return 0;
 }
 
 extern "C" int bjx_chees_metric_covariance(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, int32_t options, float* metric_state,
@@ -1173,5 +1138,5 @@ extern "C" int bjx_chees_metric_covariance(bjx_handle_t h, void* nccl_comm, int3
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   if (D > 1024) return bjx_fail(h, BJX_E_UNSUPPORTED, "ChEES is built for dim <= 1024");
   const MmLayout L = mm_layout(C, D, n_ranks, options);
-  return cov_merge(h, nccl_comm, n_ranks, L, metric_state, nullptr, out + 1 + D, out);
+  return mm_cov_merge(h, nccl_comm, n_ranks, L, metric_state, nullptr, out + 1 + D, out);
 }

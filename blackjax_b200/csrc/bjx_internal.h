@@ -32,12 +32,15 @@ void launch_ess(int T, int C, int D, const float* hist, float* ess, float* scrat
 // single-chain ESS of every (chain, dim) series: ess [C, D]; lags_out (optional, zeroed) [C] lags evaluated per chain
 void launch_ess_per_chain(int T, int C, int D, const float* hist, float* ess, int* lags_out, cudaStream_t s);
 // windowed D x D covariance accumulators of bjx_adapt.cu: cov_stat_blocks(C) blocks of cov_block_floats(D) floats (count,
-// -, mean[D], m2[D, D] lower triangle); the fold uses nb * (2 + 2D) floats of stats scratch; the merge writes the full
-// covariance m2 / max(n - 1, 1) [D, D] to out and (n, mean[D]) to count_mean
+// -, mean[D], m2[D, D] lower triangle).  launch_block_stats writes the nb records (sum acc, n, mean[D], M2[D]) of the
+// statistic blocks of x [C, D] to out; the fold takes these records of q as stats.  The merge of nblk accumulators writes
+// the full covariance m2 / max(n - 1, 1) [D, D], whitened by imm unless it is null, to out and (n, mean[D]) to count_mean
+// unless it is null.
 int cov_stat_blocks(int C);
 size_t cov_block_floats(int D);
-void launch_cov_fold(int C, int D, const float* q, float* stats, float* cov, cudaStream_t s);
-void launch_cov_merge(int C, int D, const float* cov, float* out, float* count_mean, cudaStream_t s);
+void launch_block_stats(int C, int D, const float* x, const float* acc, float* out, cudaStream_t s);
+void launch_cov_fold(int C, int D, const float* q, const float* stats, float* cov, cudaStream_t s);
+void launch_cov_merge(int nblk, int D, const float* cov, const float* imm, float* out, float* count_mean, cudaStream_t s);
 }  // namespace bjx
 
 // Host-side routing and run-loop helpers of bjx_api.cu, shared with the entry points of other translation units.

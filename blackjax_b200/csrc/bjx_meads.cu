@@ -925,8 +925,10 @@ extern "C" int bjx_meads_lrd_update(bjx_handle_t h, const float* q, const float*
   BJX_CHECK_LAUNCH("k_meads_gram");
   // this step's metric (:549-568)
   if (in_window) {
+    // k_block_stats also sums an acceptance array over each block; q stands in for it (that sum is not read here)
+    launch_block_stats(C, D, q, q, ls + L.stats, s);
     launch_cov_fold(C, D, q, ls + L.stats, ls + L.cov, s);
-    launch_cov_merge(C, D, ls + L.cov, ls + L.W, ls + L.cm, s);
+    launch_cov_merge(cov_stat_blocks(C), D, ls + L.cov, nullptr, ls + L.W, ls + L.cm, s);
     BJX_CHECK_LAUNCH("launch_cov_merge");
   }
   k_lrd_fallback<<<1, 512, 0, s>>>(D, k, K, n, mu, sd, in_window ? 1 : 0, ls + L.cm, ls, ls + L.sigma, ls + L.U, ls + L.lam);
@@ -962,7 +964,7 @@ extern "C" int bjx_meads_lrd_metric(bjx_handle_t h, float* lrd_state, const floa
   cudaStream_t s = h->stream;
   // the last accumulator if it holds 2 D samples, else the fallback on the final positions (:746-771)
   k_meads_moments<<<dim3((D + 31) / 32, 1), dim3(32, 8), 0, s>>>(C, D, final_q, fin, fin + D, fin + 2 * D);
-  launch_cov_merge(C, D, ls + L.cov, ls + L.W, ls + L.cm, s);
+  launch_cov_merge(cov_stat_blocks(C), D, ls + L.cov, nullptr, ls + L.W, ls + L.cm, s);
   k_lrd_fallback<<<1, 512, 0, s>>>(D, k, 1, C, fin, fin + D, 1, ls + L.cm, ls, ls + L.sigma, ls + L.U, ls + L.lam);
   BJX_CHECK_LAUNCH("k_lrd_fallback");
   rc = lrd_eigensolve(h, k, 1, L, ls);

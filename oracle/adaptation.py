@@ -5,7 +5,7 @@ TEST INFRASTRUCTURE (see oracle/__init__.py).  float32.
 Follows:
 * dual averaging   blackjax/optimizers/dual_averaging.py:87-129, adaptation/step_size.py:65-150
 * Welford / IMM    blackjax/adaptation/mass_matrix.py:364-444 (welford), :335-357 (regularised final)
-* CGL merge        blackjax/adaptation/metric_buffers.py:334-393 (cgl_merge_two)
+* CGL merge        blackjax/adaptation/metric_buffers.py:334-393 (cgl_merge_two), :396-450 (cgl_update_batch)
 * schedule         blackjax/adaptation/staged_adaptation.py:315-405 (build_schedule)
 * engine           blackjax/adaptation/staged_adaptation.py:111-307 (_make_engine), :731-754 (one_step),
                    :864-874 (single-chain run), :906-966 (multi-chain shared-epsilon run)
@@ -107,6 +107,34 @@ def cgl_merge(a, b):
     c = F(a.n * b.n / n_ab)
     cross = delta * delta * c if a.m2.ndim == 1 else np.outer(delta, delta) * c
     return Welford(mean, (a.m2 + b.m2 + cross).astype(F), n_ab)
+
+
+# ---- full moment block (metric_buffers.py:396-450) ------------------------------------------------------------------
+# The same Chan-Golub-LeVeque merge as cgl_merge, kept apart because the arithmetic differs: cgl_update_batch keeps the
+# count as a float32 (rounded once it passes 2^24) and forms its factors in float32, where cgl_merge takes integer counts
+# and rounds each factor once.
+class MomentBlock(NamedTuple):
+    count: np.float32
+    mean: np.ndarray
+    m2: np.ndarray
+
+
+def moment_block_init(D):
+    return MomentBlock(F(0.0), np.zeros(D, F), np.zeros((D, D), F))
+
+
+def cgl_update_batch(block, batch):
+    batch = np.asarray(batch, F)
+    n_a, n_b = block.count, F(batch.shape[0])
+    mean_b = np.mean(batch, axis=0, dtype=F).astype(F)
+    cb = (batch - mean_b).astype(F)
+    m2_b = (cb.T @ cb).astype(F)
+    n_ab = F(n_a + n_b)
+    safe = n_ab if n_ab > 0 else F(1.0)
+    delta = (mean_b - block.mean).astype(F)
+    mean = (block.mean + delta * F(n_b / safe)).astype(F)
+    m2 = (block.m2 + m2_b + np.outer(delta, delta).astype(F) * F(n_a * n_b / safe)).astype(F)
+    return MomentBlock(n_ab, mean, m2)
 
 
 def batch_block(x):

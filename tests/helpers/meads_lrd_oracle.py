@@ -1,8 +1,7 @@
 """Restatement of BlackJAX's MEADS-LRD statistics (``meads_adaptation(..., low_rank_rank=k)``): the shared low-rank
 momentum metric of one warm-up step, and the fold parameters computed under it.
 
-TEST INFRASTRUCTURE, float32, built on oracle/meads.py (left unchanged) and the moment block of
-tests/helpers/chees_metric_oracle.py.
+TEST INFRASTRUCTURE, float32, built on oracle/meads.py (left unchanged) and the moment block of oracle/adaptation.py.
 
 Follows blackjax/adaptation/meads_adaptation.py and metric_estimators.py:
 * accumulated metric         metric_estimators.py:543-615   cov = m2 / max(count - 1, 1), sigma = sqrt(max(diag, 0)) with
@@ -18,9 +17,8 @@ Follows blackjax/adaptation/meads_adaptation.py and metric_estimators.py:
 import numpy as np
 
 from oracle import meads as omeads
+from oracle.adaptation import MomentBlock, cgl_update_batch, moment_block_init  # noqa: F401  (re-exported)
 from oracle.hmc import F
-
-from chees_metric_oracle import MomentBlock, cgl_update_batch, moment_block_init  # noqa: F401  (re-exported)
 
 LAM_FLOOR = F(1e-6)
 

@@ -1,5 +1,5 @@
 """GPU tests of ChEES with mass_matrix_estimation="diagonal": the SYRK covariance accumulator against float64 numpy, the
-device update teacher-forced against tests/helpers/chees_metric_oracle.py, bit-identity with the identity path when the
+device update teacher-forced against oracle/chees.py, bit-identity with the identity path when the
 window never opens, the statistics of a warm-up on a target a diagonal metric cannot whiten, and independence of the GPU
 count."""
 import math
@@ -15,12 +15,10 @@ import blackjax_b200 as bj
 from blackjax_b200 import _engine, targets as T
 from blackjax_b200._lib import CHEES_LENGTH_FLOOR, CHEES_WHITEN, check, lib, ptr
 from blackjax_b200.adaptation.chees_adaptation import adam
+from oracle import adaptation as oadapt
 from oracle import chees as ochees
 from oracle import prng as oprng
 from oracle import targets as otargets
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import chees_metric_oracle as ocm  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -95,20 +93,20 @@ def test_chees_update_metric_teacher_forced_vs_oracle(D):
     check(L_.bjx_chees_metric_init(eng.h, ptr(ms), 1, OPTS, ptr(imm)), eng.h)
     eng._imm, eng._imm_key = imm, (imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device))
     os_ = ochees.chees_init(0.05)
-    wf, cov, eig = ocm.welford_init(D), ocm.moment_block_init(D), ocm.eig_state_init(D)
-    thresh = ocm.engagement_threshold(D)
+    wf, cov, eig = oadapt.welford_init(D), oadapt.moment_block_init(D), ochees.eig_state_init(D)
+    thresh = ochees.engagement_threshold(D)
     keys = bj.random.split(bj.random.key(5, DEV), T_)
     near_integer = 0
     n64, mean64, m2_64 = 0, np.zeros(D), np.zeros(D)
     for t in range(T_):
-        imm_or = ocm.diagonal_imm(wf, thresh, D)
+        imm_or = ochees.diagonal_imm(wf, thresh, D)
         imm_dev = npy(imm)
         # imm against the same window's float64 moments; the oracle's row-by-row float32 fold (up to 230k rows) drifts
         # from them by a few 1e-5, so it is held to 1e-4
         imm64 = np.maximum(m2_64 / (n64 - 1), 1e-20) if n64 >= thresh else np.ones(D)
         np.testing.assert_allclose(imm_dev, imm64, rtol=1e-5)
         np.testing.assert_allclose(imm_or, imm64, rtol=1e-4)
-        consumed, _ = ocm.apply_length_floor(os_.trajectory_length, eig.lambda_max, wf.n >= thresh, True, 1000, os_.step_size)
+        consumed, _ = ochees.apply_length_floor(os_.trajectory_length, eig.lambda_max, wf.n >= thresh, True, 1000, os_.step_size)
         L_or = ochees.integration_steps(os_.random_generator_arg, F(consumed / os_.step_size), 1.0, max_bits)
         x = float(ochees.jitter(os_.random_generator_arg, 1.0, max_bits)) * float(consumed / os_.step_size)
         L_dev = int(steps_c[0])
@@ -124,8 +122,8 @@ def test_chees_update_metric_teacher_forced_vs_oracle(D):
                                          ptr(info.is_divergent.to(torch.uint8)), 0.1, 0.9, 0.999, 0.651, 0.5, 1000,
                                          int(in_window), int(recompute), ptr(eps_c), ptr(steps_c), None, ptr(imm), ptr(lam),
                                          ptr(engd)), eng.h)
-        os_ = ocm.chees_update(os_, npy(info.proposal.position), npy(info.proposal.momentum), npy(init_q),
-                               npy(info.acceptance_rate), npy(info.is_divergent), imm=imm_dev, lr=0.1, max_bits=max_bits)
+        os_ = ochees.chees_update(os_, npy(info.proposal.position), npy(info.proposal.momentum), npy(init_q),
+                                  npy(info.acceptance_rate), npy(info.is_divergent), imm=imm_dev, lr=0.1, max_bits=max_bits)
         newq = npy(state.position)
         if in_window:
             b64 = newq.astype(np.float64)
@@ -134,10 +132,10 @@ def test_chees_update_metric_teacher_forced_vs_oracle(D):
             n_ab = n64 + C
             m2_64 = m2_64 + ((b64 - mb) ** 2).sum(0) + delta * delta * (n64 * C / n_ab)
             mean64, n64 = mean64 + delta * (C / n_ab), n_ab
-            wf = ocm.welford_fold(wf, newq)
-            cov = ocm.cgl_update_batch(cov, newq)
+            wf = ochees.welford_fold(wf, newq)
+            cov = oadapt.cgl_update_batch(cov, newq)
             if recompute:
-                eig = ocm.recompute_eig(cov, imm_dev, eig)
+                eig = ochees.recompute_eig(cov, imm_dev, eig)
         hdr = npy(st[:16])
         np.testing.assert_allclose(hdr[[0, 2]], [os_.step_size, os_.trajectory_length], rtol=1e-5)
         assert bool(npy(engd)[t]) == (wf.n >= thresh), t
@@ -198,7 +196,7 @@ def test_chees_diagonal_statistics_slow_direction():
     top = np.linalg.eigvalsh(cov / sd[:, None] / sd[None, :])[-1]
     lam = float(info.lambda_max[-1])
     eps, n_lf = params["step_size"], params["integration_steps_params"][0]
-    r = ocm.chees_run(otgt, oprng.key(21), q, 0.05, lr=0.05, num_steps=steps, mass_matrix_estimation="diagonal")
+    r = ochees.chees_run(otgt, oprng.key(21), q, 0.05, lr=0.05, num_steps=steps, mass_matrix_estimation="diagonal")
     print(f"device eps {eps:.4f} n_lf {n_lf:.2f} lambda {lam:.2f}; oracle eps {float(r.step_size):.4f} "
           f"n_lf {float(r.num_leapfrog_steps):.2f} lambda {float(r.lambda_max):.2f}; top eigenvalue {top:.2f}")
     assert abs(lam / top - 1) < 0.10
