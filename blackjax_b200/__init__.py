@@ -13,6 +13,7 @@ from .adaptation.window_adaptation import build_schedule, window_adaptation  # n
 from .adaptation.chees_adaptation import chees_adaptation  # noqa: F401
 from .adaptation.meads_adaptation import meads_adaptation  # noqa: F401
 from .adaptation.mclmc_adaptation import MCLMCAdaptationState, mclmc_find_L_and_step_size  # noqa: F401
+from .adaptation.adjusted_mclmc_adaptation import adjusted_mclmc_find_L_and_step_size  # noqa: F401
 from .base import AdaptationAlgorithm, AdaptationResults, GenerateSamplingAPI, SamplingAlgorithm  # noqa: F401
 from . import mcmc  # noqa: F401
 from .mcmc import hmc as _hmc

@@ -292,13 +292,18 @@ class Engine:
         qo, lo, go = out if out is not None else (torch.empty_like(q), torch.empty_like(logp), torch.empty_like(g))
         eps, eps_dev = self._eps(step_size)
         info = self._info(info_fields or {})
-        steps_dev = None
-        if isinstance(num_integration_steps, torch.Tensor):  # adjusted_mclmc_dynamic: one step count per chain
+        steps_dev = avg_dev = None
+        if isinstance(num_integration_steps, torch.Tensor) and num_integration_steps.is_floating_point():
+            avg_dev = _f32(num_integration_steps.to(self.device, torch.float32).contiguous(), (self.C,),
+                           "num_integration_steps")  # ceil per chain
+            num_integration_steps = 0
+        elif isinstance(num_integration_steps, torch.Tensor):  # adjusted_mclmc_dynamic: one step count per chain
             steps_dev = num_integration_steps.to(device=self.device, dtype=torch.int32).contiguous()
             if steps_dev.shape != (self.C,):
                 raise ValueError(f"per-chain num_integration_steps must have shape ({self.C},)")
             num_integration_steps = 0
         check(lib().bjx_set_integration_steps(self.h, ptr(steps_dev)), self.h)
+        check(lib().bjx_set_integration_steps_avg(self.h, ptr(avg_dev)), self.h)
         try:
             check(lib().bjx_adjusted_mclmc_step(self.h, ptr(keys), ptr(q), ptr(logp), ptr(g), ptr(qo), ptr(lo), ptr(go),
                                                 eps, ptr(eps_dev), int(num_integration_steps), float(L_proposal_factor),
@@ -306,8 +311,24 @@ class Engine:
         finally:
             if steps_dev is not None:
                 check(lib().bjx_set_integration_steps(self.h, None), self.h)
-        self._amclmc_keepalive = (steps_dev, eps_dev)  # the launch is asynchronous: keep the arrays until the next call
+            if avg_dev is not None:
+                check(lib().bjx_set_integration_steps_avg(self.h, None), self.h)
+        self._amclmc_keepalive = (steps_dev, eps_dev, avg_dev)  # the launch is asynchronous: keep the arrays
         return qo, lo, go
+
+    def adjusted_mclmc_num_steps(self, device_rule, avg, random_generator_arg):
+        """The step counts int32 [C] of a dynamic rule ``device_rule = (rule, min_steps)`` at a per-chain ``avg`` [C]
+        (libbjx ``bjx_adjusted_mclmc_num_steps``); random_generator_arg [C, 2] is read, not advanced.  The fixed rule
+        clips at 1, as make_random_trajectory_length_fn(False) does."""
+        rule, min_steps = device_rule
+        if rule == _lib.AMCLMC_STEPS_FIXED:
+            min_steps = max(int(min_steps), 1)
+        avg = _f32(avg.to(self.device, torch.float32).contiguous(), (self.C,), "avg_num_integration_steps")
+        rga = random_generator_arg.to(self.device).contiguous()
+        out = torch.empty(self.C, dtype=torch.int32, device=self.device)
+        check(lib().bjx_adjusted_mclmc_num_steps(self.h, int(rule), ptr(avg), int(min_steps), ptr(rga), ptr(out)), self.h)
+        self._num_steps_keepalive = (avg, rga)
+        return out
 
     def nuts_last_stats(self):
         a, b = C.c_int64(), C.c_int64()

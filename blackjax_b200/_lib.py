@@ -89,6 +89,15 @@ _SIGNATURES = {
     "bjx_adjusted_mclmc_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_float, C.c_int32,
                                             C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_int32, _f32p, C.c_int32, _f32p,
                                             C.c_void_p]),
+    "bjx_set_integration_steps_avg": (C.c_int, [C.c_void_p, _f32p]),
+    "bjx_adjusted_mclmc_num_steps": (C.c_int, [C.c_void_p, C.c_int32, _f32p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "bjx_adjusted_mclmc_tune_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_void_p, C.c_int32, C.c_int32,
+                                               _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_float,
+                                               C.c_void_p, C.c_void_p]),
+    "bjx_adjusted_mclmc_find_l_and_step_size": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_void_p, C.c_int32,
+                                                          C.c_int32, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32,
+                                                          C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_float, C.c_float,
+                                                          C.c_double, C.c_int64, _f32p]),
     "bjx_nuts_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
                                 C.c_int32, C.POINTER(Info), _f32p, _f32p]),
     "bjx_nuts_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, C.c_int32, _f32p,

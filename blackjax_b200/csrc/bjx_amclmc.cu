@@ -28,6 +28,7 @@ static int amclmc_transition(bjx_handle_t h, const uint32_t* keys, const float* 
   a.logp_out = logp_out;
   a.g_out = grad_out;
   a.amclmc = A;
+  a.amclmc.avg = h->steps_avg;
   if (info) {
     a.info.acceptance_rate = info->acceptance_rate;
     a.info.is_accepted = info->is_accepted;

@@ -220,6 +220,14 @@ extern "C" int bjx_set_integration_steps(bjx_handle_t h, const int32_t* steps_de
   return 0;
 }
 
+// Adjusted MCLMC with a per-chain average trajectory length float32 [C] (device), e.g. the tuner's L / step_size, for the
+// following bjx_adjusted_mclmc_step / bjx_adjusted_mclmc_sample calls; NULL restores the scalar arguments.
+extern "C" int bjx_set_integration_steps_avg(bjx_handle_t h, const float* avg_dev) {
+  if (!h) return bjx_fail(h, BJX_E_INVALID, "null handle");
+  h->steps_avg = avg_dev;
+  return 0;
+}
+
 // Generalized HMC's slice noise (blackjax/mcmc/ghmc.py:90,172 `noise_fn(key_noise)`): per-chain values float32 [C]
 // (device) added to the slice translation of the following bjx_ghmc_step calls; NULL restores the default (0).
 extern "C" int bjx_set_ghmc_noise(bjx_handle_t h, const float* noise_dev) {

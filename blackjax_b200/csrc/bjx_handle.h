@@ -3,6 +3,7 @@
 #include <string>
 
 #include "../../include/bjx.h"
+#include "bjx_internal.h"
 #include "bjx_kernels.cuh"
 
 namespace bjx {
@@ -52,6 +53,7 @@ struct bjx_handle_s {
   bool general_integrator = false;
   int key_shared = 0;                  // see bjx_set_key_mode
   const int32_t* steps_dev = nullptr;  // see bjx_set_integration_steps
+  const float* steps_avg = nullptr;    // see bjx_set_integration_steps_avg
   const float* ghmc_noise = nullptr;   // see bjx_set_ghmc_noise
   uint32_t chain_offset = 0;
   uint32_t* sample_keys = nullptr;     // [num_steps, 2] step keys of the run loops (bjx_hmc_sample, ...)
@@ -87,6 +89,25 @@ struct SharedStepKeys {
   ~SharedStepKeys() { h->key_shared = saved; }
 };
 
+inline unsigned blocks_for(long long n, int per_block) { return (unsigned)((n + per_block - 1) / per_block); }
+
+// Stream-ordered device scratch of one call, released on the stream when it goes out of scope.
+struct StreamScratch {
+  bjx_handle_t h;
+  void* ptr = nullptr;
+  explicit StreamScratch(bjx_handle_t h_) : h(h_) {}
+  ~StreamScratch() {
+    if (ptr) cudaFreeAsync(ptr, h->stream);
+  }
+};
+
+// Chains per slice of the tuners' ESS stage: the most whose position history [n, slice, D] fits max_history_bytes, at least
+// one and at most C.
+inline long long history_slice_chains(long long max_history_bytes, int n, int D, int C) {
+  long long cs = max_history_bytes / ((long long)n * D * (long long)sizeof(float));
+  return cs < 1 ? 1 : (cs > C ? C : cs);
+}
+
 // Error idiom of every entry point: a failing CUDA call or kernel launch returns its cudaError_t, message in h->err.
 #define BJX_CUDA(call)                                            \
   do {                                                            \
@@ -98,3 +119,27 @@ struct SharedStepKeys {
     cudaError_t e_ = cudaGetLastError();                          \
     if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, where);    \
   } while (0)
+
+// The tuners' ESS stage, one slice of chains [c0, c0 + n) at a time: n_steps calls of step(c0, n, t), each followed by a
+// copy of the slice's positions q into history row t; then the per-chain ESS of the slice into ess [n, D] and
+// finish(c0, n).  history holds [n_steps, cs, D] floats, ess [cs, D].
+template <class Step, class Finish>
+int run_ess_slices(bjx_handle_t h, long long cs, int n_steps, const float* q, float* history, float* ess, Step step,
+                   Finish finish) {
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  for (long long c0 = 0; c0 < C; c0 += cs) {
+    const int n = (int)((C - c0) < cs ? (C - c0) : cs);
+    const size_t row = (size_t)c0 * D;
+    for (int t = 0; t < n_steps; ++t) {
+      int rc = step(c0, n, t);
+      if (rc) return rc;
+      BJX_CUDA(cudaMemcpyAsync(history + (size_t)t * n * D, q + row, sizeof(float) * n * D, cudaMemcpyDeviceToDevice,
+                               h->stream));
+    }
+    bjx::launch_ess_per_chain(n_steps, n, D, history, ess, nullptr, h->stream);
+    BJX_CHECK_LAUNCH("k_ess_chain");
+    int rc = finish(c0, n);
+    if (rc) return rc;
+  }
+  return 0;
+}

@@ -31,6 +31,11 @@ size_t ess_scratch_floats(int T, int C, int D);
 void launch_ess(int T, int C, int D, const float* hist, float* ess, float* scratch, cudaStream_t s);
 // single-chain ESS of every (chain, dim) series: ess [C, D]; lags_out (optional, zeroed) [C] lags evaluated per chain
 void launch_ess_per_chain(int T, int C, int D, const float* hist, float* ess, int* lags_out, cudaStream_t s);
+// the tuners' per-chain key tree (bjx_mclmc_tune.cu): part1[c], part2[c] = split(k_c) with k_c the chain's key
+// (split(keys[0:2], n_global)[chain_offset + c] when key_shared, else keys[c]); out[c] = split(base[c], n)[i]
+void launch_tune_part_keys(int C, int key_shared, uint32_t chain_offset, const uint32_t* keys, uint32_t* part1,
+                           uint32_t* part2, cudaStream_t s);
+void launch_tune_fold_keys(int C, const uint32_t* base, uint32_t i, uint32_t* out, cudaStream_t s);
 // windowed D x D covariance accumulators of bjx_adapt.cu: cov_stat_blocks(C) blocks of cov_block_floats(D) floats (count,
 // -, mean[D], m2[D, D] lower triangle).  launch_block_stats writes the nb records (sum acc, n, mean[D], M2[D]) of the
 // statistic blocks of x [C, D] to out; the fold takes these records of q as stats.  The merge of nblk accumulators writes

@@ -11,7 +11,7 @@ namespace bjx {
 
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
 enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
-               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE };
+               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE };
 
 struct LaunchArgs {
   Params P;
@@ -22,6 +22,7 @@ struct LaunchArgs {
   MclmcArgs mclmc;
   AmclmcArgs amclmc;
   MclmcTuneArgs mclmc_tune;
+  AmclmcTuneArgs amclmc_tune;
   int grid_override;    // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
@@ -120,6 +121,12 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
       if constexpr (!DM) {
         k_mclmc_tune<R, TK, DM, GEN><<<grid, block, smem, st>>>(a.P, a.keys, a.q_out, a.p_io, a.logp_out, a.g_out,
                                                                  a.mclmc_tune);
+        return 0;
+      }
+      break;
+    case K_AMCLMC_TUNE:  // diagonal metrics only, as K_MCLMC
+      if constexpr (!DM) {
+        k_amclmc_tune<R, TK, DM, GEN><<<grid, block, smem, st>>>(a.P, a.keys, a.q_out, a.logp_out, a.g_out, a.amclmc_tune);
         return 0;
       }
       break;

@@ -82,8 +82,6 @@ __global__ void k_tune_L_from_ess(int C, int D, int n3, const float* __restrict_
   if (lane == 0) L_out[c] = __fmul_rn(__fmul_rn(l_factor, eps[c]), __fdiv_rn(acc, (float)D));
 }
 
-inline unsigned blocks_for(long long n, int per_block) { return (unsigned)((n + per_block - 1) / per_block); }
-
 // the predictor's constants as the reference forms them: Python floats (double), then float32 in the jnp expressions
 struct TuneConstants {
   float dim_eev, trust6, decay;
@@ -106,17 +104,17 @@ int tune_dispatch(bjx_handle_t h, const Params& P, const uint32_t* keys, float* 
   return dispatch(h, K_MCLMC_TUNE, true, a);
 }
 
-// Stream-ordered device scratch of one call, released on the stream when it goes out of scope.
-struct StreamScratch {
-  bjx_handle_t h;
-  void* ptr = nullptr;
-  explicit StreamScratch(bjx_handle_t h_) : h(h_) {}
-  ~StreamScratch() {
-    if (ptr) cudaFreeAsync(ptr, h->stream);
-  }
-};
-
 }  // namespace
+
+namespace bjx {
+void launch_tune_part_keys(int C, int key_shared, uint32_t chain_offset, const uint32_t* keys, uint32_t* part1,
+                           uint32_t* part2, cudaStream_t s) {
+  k_tune_part_keys<<<blocks_for(C, 256), 256, 0, s>>>(C, key_shared, chain_offset, keys, part1, part2);
+}
+void launch_tune_fold_keys(int C, const uint32_t* base, uint32_t i, uint32_t* out, cudaStream_t s) {
+  k_tune_fold_keys<<<blocks_for(C, 256), 256, 0, s>>>(C, base, i, out);
+}
+}  // namespace bjx
 
 extern "C" int bjx_mclmc_tune_step(bjx_handle_t h, const uint32_t* keys, float* q, float* p, float* logp, float* grad,
                                    float* step_size, float L, const float* L_dev, float energy_cutoff, float* time,
@@ -181,8 +179,7 @@ extern "C" int bjx_mclmc_find_l_and_step_size(bjx_handle_t h, const uint32_t* rn
   const bool estimate = num_steps2 > 1, readjust = estimate && diagonal_preconditioning && readjust_steps > 0;
   const bool stage3 = num_steps3 >= 2;
   // stage 3 runs on slices of cs chains whose position history [n3, cs, D] fits the budget (at least one chain)
-  long long cs = stage3 ? max_history_bytes / ((long long)num_steps3 * D * (long long)sizeof(float)) : 0;
-  cs = cs < 1 ? 1 : (cs > C ? C : cs);
+  const long long cs = stage3 ? history_slice_chains(max_history_bytes, num_steps3, D, C) : 1;
   // scratch: part1, part2, step keys [C, 2] u32 | time, x_avg, eps_max, total, L_new [C] | moments [C, 2, D] |
   // history [n3, cs, D] | ess [cs, D]; float offsets rounded up to 4 floats keep every row 16-byte aligned
   auto up4 = [](size_t n) { return (n + 3) & ~(size_t)3; };
@@ -249,8 +246,7 @@ extern "C" int bjx_mclmc_find_l_and_step_size(bjx_handle_t h, const uint32_t* rn
   }
   if (!stage3) return 0;
   // stage 3 (:367-399), one slice of chains at a time: transitions, position history, per-chain ESS, L
-  for (long long c0 = 0; c0 < C; c0 += cs) {
-    const int n = (int)((C - c0) < cs ? (C - c0) : cs);
+  auto step = [&](long long c0, int n, int t) -> int {
     const size_t row = (size_t)c0 * D;
     LaunchArgs a{};
     a.P = P;
@@ -264,17 +260,15 @@ extern "C" int bjx_mclmc_find_l_and_step_size(bjx_handle_t h, const uint32_t* rn
     a.g_out = grad + row;
     a.mclmc.L_dev = L + c0;
     a.mclmc.energy_cutoff = energy_cutoff;
-    for (int t = 0; t < num_steps3; ++t) {
-      k_tune_fold_keys<<<blocks_for(n, 256), 256, 0, st>>>(n, part2 + 2 * c0, (uint32_t)t, step_keys);
-      BJX_CHECK_LAUNCH("k_tune_fold_keys");
-      if ((rc = dispatch(h, K_MCLMC, true, a))) return rc;
-      BJX_CUDA(cudaMemcpyAsync(history + (size_t)t * n * D, q + row, sizeof(float) * n * D, cudaMemcpyDeviceToDevice, st));
-    }
-    launch_ess_per_chain(num_steps3, n, D, history, ess, nullptr, st);
-    BJX_CHECK_LAUNCH("k_ess_chain");
+    k_tune_fold_keys<<<blocks_for(n, 256), 256, 0, st>>>(n, part2 + 2 * c0, (uint32_t)t, step_keys);
+    BJX_CHECK_LAUNCH("k_tune_fold_keys");
+    return dispatch(h, K_MCLMC, true, a);
+  };
+  auto finish = [&](long long c0, int n) -> int {
     k_tune_L_from_ess<<<blocks_for(n, kWarpsPerBlock), kThreads, 0, st>>>(n, D, num_steps3, ess, step_size + c0,
                                                                           (float)l_factor, L + c0);
     BJX_CHECK_LAUNCH("k_tune_L_from_ess");
-  }
-  return 0;
+    return 0;
+  };
+  return run_ess_slices(h, cs, num_steps3, q, history, ess, step, finish);
 }

@@ -2,6 +2,7 @@
 // dual averaging / Welford window adaptation, chain-pooled summary statistics.
 #include "bjx_internal.h"
 #include "bjx_prng.cuh"
+#include "bjx_da.cuh"
 
 namespace bjx {
 
@@ -88,20 +89,8 @@ __global__ void k_da_update(int C, float* __restrict__ st, const float* __restri
                             float* __restrict__ eps_out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float log_step = st[5 * c + 0], avg_log_step = st[5 * c + 1], step = st[5 * c + 2];
-  float avg_error = st[5 * c + 3];
-  const float mu = st[5 * c + 4];
-  const float gradient = target - acc[c];
-  const float reg_step = step + 10.f;                    // t0 = 10
-  const float eta_t = powf(step, -0.75f);                // kappa = 0.75
-  avg_error = (1.f - (1.f / reg_step)) * avg_error + gradient / reg_step;
-  const float log_x = mu - (sqrtf(step) / 0.05f) * avg_error;  // gamma = 0.05
-  const float log_x_avg = eta_t * log_step + (1.f - eta_t) * avg_log_step;  // uses the PRE-update iterate (:122)
-  st[5 * c + 0] = log_x;
-  st[5 * c + 1] = log_x_avg;
-  st[5 * c + 2] = step + 1.f;
-  st[5 * c + 3] = avg_error;
-  if (eps_out) eps_out[c] = expf(log_x);
+  da_update_step(st + 5 * c, acc[c], target);
+  if (eps_out) eps_out[c] = expf(st[5 * c + 0]);
 }
 __global__ void k_da_reset(int C, float* __restrict__ st, float* __restrict__ eps_out) {  // staged_adaptation.py:233-249
   const int c = blockIdx.x * blockDim.x + threadIdx.x;

@@ -31,8 +31,9 @@ def init(position, logdensity_fn):
 
 
 def steps_argument(num_integration_steps):
-    """The step count as the kernel takes it: an int, or an int32 tensor [C] for per-chain counts.  A non-integer scalar
-    runs ceil(n) steps, as the reference's ``fori_loop(0, n, ...)`` does with a float bound."""
+    """The step count as the kernel takes it: an int, or a tensor [C] for per-chain counts.  A non-integer scalar runs
+    ceil(n) steps, as the reference's ``fori_loop(0, n, ...)`` does with a float bound; so does a floating-point tensor
+    (e.g. the tuner's ``L / step_size``), chain by chain on the device."""
     if isinstance(num_integration_steps, torch.Tensor) and num_integration_steps.ndim >= 1:
         return num_integration_steps
     n = float(num_integration_steps)
@@ -74,6 +75,12 @@ def build_kernel(integrator=isokinetic_mclachlan, divergence_threshold: float = 
                        fields["is_divergent"].bool(), fields["energy"], proposal, num_integration_steps)
         return HMCState(qo, lo, go), info
 
+    # what adjusted_mclmc_find_L_and_step_size reads: the kernel's integrator, divergence threshold, chain offset and step
+    # rule (None: the static kernel, ceil(L / step_size) steps)
+    kernel.coefficients = coefficients
+    kernel.divergence_threshold = divergence_threshold
+    kernel.chain_offset = chain_offset
+    kernel.device_rule = None
     return kernel
 
 

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from .. import random as jr
+from .._engine import get_engine
 from .._lib import AMCLMC_STEPS_FIXED, AMCLMC_STEPS_RANDINT, AMCLMC_STEPS_UNIFORM
 from ..base import build_sampling_algorithm
 from . import adjusted_mclmc
@@ -52,17 +53,34 @@ def build_kernel(integration_steps_fn: Callable = _integration_steps, integrator
     an int32 tensor [n_chains] (or an int); ``next_random_arg_fn`` maps ``random_generator_arg`` to the next one.
     ``kw`` (full_info, inplace, chain_offset) as ``adjusted_mclmc.build_kernel``."""
     static = adjusted_mclmc.build_kernel(integrator, divergence_threshold, **kw)
+    device_rule = getattr(integration_steps_fn, "device_rule", None)
 
     def kernel(rng_key, state, logdensity_fn, step_size, L_proposal_factor=math.inf, inverse_mass_matrix=1.0,
                integration_steps_params=()):
-        num_integration_steps = integration_steps_fn(state.random_generator_arg, *integration_steps_params)
+        if device_rule is not None and device_rule[0] != AMCLMC_STEPS_RANDINT and _per_chain(integration_steps_params):
+            # a per-chain average trajectory length (the tuner's L / step_size): the rule runs on the device
+            eng = get_engine(state.position, logdensity_fn, divergence_threshold=divergence_threshold)
+            num_integration_steps = eng.adjusted_mclmc_num_steps(device_rule, integration_steps_params[0],
+                                                                 state.random_generator_arg)
+        else:
+            num_integration_steps = integration_steps_fn(state.random_generator_arg, *integration_steps_params)
         st = HMCState(state.position, state.logdensity, state.logdensity_grad)
         new, info = static(rng_key, st, logdensity_fn, step_size, (num_integration_steps,), inverse_mass_matrix,
                            L_proposal_factor)
         next_arg = next_random_arg_fn(state.random_generator_arg)
         return DynamicHMCState(new.position, new.logdensity, new.logdensity_grad, next_arg), info
 
+    kernel.coefficients = static.coefficients
+    kernel.divergence_threshold = divergence_threshold
+    kernel.chain_offset = static.chain_offset
+    kernel.device_rule = device_rule
+    kernel.dynamic = True
     return kernel
+
+
+def _per_chain(integration_steps_params):
+    return (len(integration_steps_params) == 1 and isinstance(integration_steps_params[0], torch.Tensor)
+            and integration_steps_params[0].ndim >= 1)
 
 
 def as_top_level_api(logdensity_fn, step_size, L_proposal_factor=math.inf, inverse_mass_matrix=1.0, *,
@@ -103,7 +121,8 @@ def trajectory_length(t, mu):
 def make_random_trajectory_length_fn(random_trajectory_length: bool, *, min_steps: int = 1) -> Callable:
     """blackjax/mcmc/adjusted_mclmc_dynamic.py:215-247: ``(random_generator_arg, avg_num_integration_steps) -> int32``.
     Random: ``max(ceil(uniform(key) * rescale(avg)), min_steps)`` per chain (the reference clips at 1; ``min_steps=0`` is
-    the unclipped rule of its own sampling tests).  Otherwise ``max(ceil(avg), 1)`` for every chain."""
+    the unclipped rule of its own sampling tests).  Otherwise ``max(ceil(avg), 1)`` for every chain.  A per-chain ``avg``
+    tensor [C] (the tuner's ``L / step_size``) is evaluated on the device by the kernels that take this rule."""
     if random_trajectory_length:
         def integration_steps_fn(key, avg_num_integration_steps):
             u = jr.uniform(key)

@@ -98,13 +98,14 @@ def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_s
     transition.  Other step-count functions go through the step API.  Returns (final state, positions
     [num_steps // thin, C, D] or None, acceptance rates [num_steps, C], step counts int32 [num_steps, C])."""
     from ._engine import get_engine
-    from ._lib import AMCLMC_STEPS_FIXED, AMCLMC_STEPS_UNIFORM, check, lib, ptr
+    from ._lib import AMCLMC_STEPS_FIXED, AMCLMC_STEPS_RANDINT, AMCLMC_STEPS_UNIFORM, check, lib, ptr
     from .mcmc import adjusted_mclmc_dynamic, integrators
     from .mcmc.dynamic_hmc import DynamicHMCState
     from .mcmc.hmc import HMCState
     from .mcmc.mclmc import metric_tensor
     dynamic = isinstance(state, DynamicHMCState)
     rule, min_steps, n, scale, rga = AMCLMC_STEPS_FIXED, 0, 0, 0.0, None
+    avg_dev = None  # a per-chain average trajectory length [C], evaluated by the kernel chain by chain
     if dynamic:
         fn = integration_steps_fn or adjusted_mclmc_dynamic._integration_steps
         if getattr(fn, "device_rule", None) is None:
@@ -112,7 +113,11 @@ def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_s
                              "make_random_trajectory_length_fn(...) on the device; use the step API for other "
                              "integration_steps_fn")
         rule, min_steps = fn.device_rule
-        if rule == AMCLMC_STEPS_FIXED:
+        if rule != AMCLMC_STEPS_RANDINT and adjusted_mclmc_dynamic._per_chain(integration_steps_params):
+            avg_dev = integration_steps_params[0].to(state[0].device, torch.float32).contiguous()
+            if rule == AMCLMC_STEPS_FIXED:
+                min_steps = max(int(min_steps), 1)  # max(ceil(avg), 1)
+        elif rule == AMCLMC_STEPS_FIXED:
             n = fn(None, *integration_steps_params)
         elif rule == AMCLMC_STEPS_UNIFORM:
             (avg,) = integration_steps_params
@@ -126,6 +131,10 @@ def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_s
             raise ValueError("the static sampler needs num_integration_steps")
         from .mcmc.adjusted_mclmc import steps_argument
         n = steps_argument(num_integration_steps)
+        if isinstance(n, torch.Tensor):
+            if not n.is_floating_point():
+                raise ValueError("the native loop takes an int or a float per-chain num_integration_steps")
+            avg_dev, n = n.to(state[0].device, torch.float32).contiguous(), 0
         q, logp, g = (t.clone() for t in state)
     eng = get_engine(q, logdensity_fn, divergence_threshold=divergence_threshold)
     eng.set_integrator(integrators.as_coefficients(integrator))
@@ -139,9 +148,18 @@ def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_s
     acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
     steps = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
     eps, eps_dev = eng._eps(step_size)
-    check(lib().bjx_adjusted_mclmc_sample(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev),
-                                          float(L_proposal_factor), int(rule), int(n), scale, int(min_steps), ptr(rga),
-                                          int(num_steps), ptr(hist), int(thin), ptr(acc), ptr(steps)), eng.h)
+    if avg_dev is not None and tuple(avg_dev.shape) != (C,):
+        raise ValueError(f"per-chain average trajectory lengths must have shape ({C},)")
+    check(lib().bjx_set_integration_steps_avg(eng.h, ptr(avg_dev)), eng.h)
+    try:
+        check(lib().bjx_adjusted_mclmc_sample(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev),
+                                              float(L_proposal_factor), int(rule), int(n), scale, int(min_steps),
+                                              ptr(rga), int(num_steps), ptr(hist), int(thin), ptr(acc), ptr(steps)),
+              eng.h)
+    finally:
+        if avg_dev is not None:
+            check(lib().bjx_set_integration_steps_avg(eng.h, None), eng.h)
+            eng._avg_keepalive = avg_dev  # the launches are asynchronous
     final = DynamicHMCState(q, logp, g, rga) if dynamic else HMCState(q, logp, g)
     return final, hist, acc, steps
 

@@ -134,6 +134,12 @@ int bjx_set_key_mode(bjx_handle_t h, int32_t shared_step_key, uint32_t chain_off
  * [n_chains] device array read by the following bjx_hmc_step / bjx_mhmc_step calls (their scalar L is then ignored);
  * NULL restores the scalar.  The caller keeps the array alive until those calls have run.  dim <= 1024 only. */
 int bjx_set_integration_steps(bjx_handle_t h, const int32_t* steps_dev);
+/* Adjusted MCLMC with one average trajectory length per chain (e.g. the tuner's L / step_size): float32 [n_chains] device
+ * array read by the following bjx_adjusted_mclmc_step / bjx_adjusted_mclmc_sample calls.  BJX_AMCLMC_STEPS_FIXED then runs
+ * ceil(avg[c]) steps (in place of num_integration_steps and bjx_set_integration_steps), BJX_AMCLMC_STEPS_UNIFORM scales by
+ * rescale(avg[c]) in float32 (in place of steps_scale); RANDINT ignores it.  NULL restores the scalar arguments.  The caller
+ * keeps the array alive until those calls have run. */
+int bjx_set_integration_steps_avg(bjx_handle_t h, const float* avg_dev);
 /* Generalized HMC slice noise (mcmc/ghmc.py:90,172 `noise_fn(key_noise)`, key_noise = split(rng_key)[1]): per-chain values
  * float32 [C] (device) for the following bjx_ghmc_step calls, evaluated by the caller; NULL = the default noise_fn (0). */
 int bjx_set_ghmc_noise(bjx_handle_t h, const float* noise_dev);
@@ -373,6 +379,54 @@ int bjx_adjusted_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q,
                               int32_t num_integration_steps, float steps_scale, int32_t min_steps,
                               uint32_t* random_generator_arg, int32_t num_steps, float* history, int32_t thin,
                               float* acceptance_history, int32_t* steps_history);
+/* The step count int32 [C] of steps_rule for every chain, as the transitions evaluate it, from avg [C] (fixed: ceil(avg),
+ * uniform: rescale(avg); randint: unused, may be NULL) and random_generator_arg [C, 2] (unused by the fixed rule, not
+ * advanced): max(rule, min_steps). */
+int bjx_adjusted_mclmc_num_steps(bjx_handle_t h, int32_t steps_rule, const float* avg, int32_t min_steps,
+                                 const uint32_t* random_generator_arg, int32_t* steps_out);
+
+/* ---- Adjusted MCLMC tuning: adjusted_mclmc_find_L_and_step_size (blackjax/adaptation/adjusted_mclmc_adaptation.py:26-507)
+ * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
+ * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_adjusted_mclmc_step (BJX_E_UNSUPPORTED
+ * otherwise).  The kernel being tuned is adjusted_mclmc (random_generator_arg NULL: ceil(L / step_size) steps, reported as
+ * the float L / step_size) or adjusted_mclmc_dynamic (random_generator_arg [C, 2], advanced in place, with steps_rule and
+ * min_steps as in bjx_adjusted_mclmc_sample and avg = L / step_size per chain); L_proposal_factor is inf. */
+/* One tuning step (dual_avg_step, adjusted_mclmc_adaptation.py:236-311) in place, for every chain.  keys (per
+ * bjx_set_key_mode) drive one transition with the handle's metric at avg = L / step_size.  A chain whose output position is
+ * not finite keeps its whole previous state, random_generator_arg included; otherwise its state is nan_to_num of the new
+ * one (a rejected transition leaves the stored rows as they are).  da_state [C, 5] (log_step, log_step_avg, step,
+ * avg_error, mu) takes one dual-averaging update on the acceptance rate toward target, kept only where mask = 1; then
+ * step = clamp(1e-5, exp(log_step), L / 1.1) and log_step = log(step).  With mask = 0, total [C] and moments [C, 2, D]
+ * (16-byte aligned) take the streaming average of (x, x^2) with weight success * step (incremental_value_update,
+ * util.py:291-319); with mask = 1 they are not touched (the reference's update is the identity there for total = 0).  With
+ * mask = 1 step_size becomes step and, unless fix_L, L becomes L * (step / old step size).  count [C] (optional) adds the
+ * transition's num_integration_steps.  success (optional) [C] uint8: the output position was finite; steps (optional) [C]
+ * int32: the integration steps run. */
+int bjx_adjusted_mclmc_tune_step(bjx_handle_t h, const uint32_t* keys, float* q, float* logp, float* grad,
+                                 uint32_t* random_generator_arg, int32_t steps_rule, int32_t min_steps, float* step_size,
+                                 float* L, float* da_state, float* total, float* moments, float* count, int32_t mask,
+                                 int32_t fix_L, float target, uint8_t* success, int32_t* steps);
+/* adjusted_mclmc_find_L_and_step_size, all windows and stages on the handle's stream with no host synchronisation.  rng_key
+ * per bjx_set_key_mode: one key [2] (chain c: split(rng_key, n_global)[chain_offset + c]) or per-chain keys [C, 2].  The
+ * host computes the stage lengths after frac /= num_windows: num_steps1 = int(N frac_tune1), num_steps2 = int(N frac_tune2),
+ * num_steps3 = int(N frac_tune3) or 0 when frac_tune3 = 0.  step_size [C], L [C] and inverse_mass_matrix [C, D] (a per-chain
+ * diagonal metric, used in place of the handle's, which must still be a diagonal kind) are the initial parameters in and
+ * the tuned ones out; L enters and leaves pinned to target_num_integration_steps * step_size.  Each window runs pass 1
+ * (num_steps1 + num_steps2 tuning steps, L fixed, the moments over the last num_steps2), and if num_steps2 != 0 the
+ * variance step (L and step_size scaled by clamp(0, contract(var) / L, 2), contract = sqrt(sum var) * tuning_factor, or
+ * sqrt(max var * D) * tuning_factor with use_max; inverse_mass_matrix = var with diagonal_preconditioning) and pass 2
+ * (num_steps1 steps, L tracking the step size).  If num_steps3 >= 2, each window then runs num_steps3 transitions and sets
+ * L = min(l_factor * L / r, 2 L) with r the per-chain ESS (mean over dimensions, or min with use_max) per transition, on
+ * slices of chains whose history [num_steps3, slice, D] fits max_history_bytes (at least one chain; the result does not
+ * depend on the slice size), followed by a pass 1 with num_steps2 = 0.  num_integration_steps [C] receives the summed
+ * num_integration_steps of every tuning transition. */
+int bjx_adjusted_mclmc_find_l_and_step_size(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, float* grad,
+                                            uint32_t* random_generator_arg, int32_t steps_rule, int32_t min_steps,
+                                            float* step_size, float* L, float* inverse_mass_matrix, int32_t num_windows,
+                                            int32_t num_steps1, int32_t num_steps2, int32_t num_steps3, float target,
+                                            int32_t diagonal_preconditioning, int32_t use_max, float tuning_factor,
+                                            float target_num_integration_steps, double l_factor, int64_t max_history_bytes,
+                                            float* num_integration_steps);
 
 /* ---- PRNG (jax.random restated; keys raw uint32 pairs) ----------------------------------------- */
 /* h may be NULL for the PRNG entry points: current device, and the stream this thread registered with
