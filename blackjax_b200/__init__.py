@@ -10,6 +10,7 @@ import functools as _functools
 from . import diagnostics, random, targets, util  # noqa: F401
 from ._lib import BjxError  # noqa: F401
 from .adaptation.window_adaptation import build_schedule, window_adaptation  # noqa: F401
+from .adaptation.low_rank_adaptation import build_growing_window_schedule, window_adaptation_low_rank  # noqa: F401
 from .adaptation.chees_adaptation import chees_adaptation  # noqa: F401
 from .adaptation.meads_adaptation import meads_adaptation  # noqa: F401
 from .adaptation.mclmc_adaptation import MCLMCAdaptationState, mclmc_find_L_and_step_size  # noqa: F401

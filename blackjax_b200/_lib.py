@@ -156,6 +156,14 @@ _SIGNATURES = {
     "bjx_meads_lrd_update": (C.c_int, [C.c_void_p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                        _f32p, _f32p, _f32p]),
     "bjx_meads_lrd_metric": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p]),
+    "bjx_lowrank_window_state_floats": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "bjx_lowrank_window_init": (C.c_int, [C.c_void_p, _f32p, C.c_float, _f32p]),
+    "bjx_lowrank_window_update": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_int32, C.c_float, C.c_float,
+                                            C.c_float, _f32p, _f32p]),
+    "bjx_lowrank_window_run": (C.c_int, [C.c_void_p, _f32p, C.c_char_p, C.c_int32, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                         C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, _f32p, _f32p, C.c_void_p,
+                                         C.c_void_p]),
+    "bjx_lowrank_window_final": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p]),
     "bjx_maximum_eigenvalue_scratch_floats":(C.c_size_t, [C.c_int64, C.c_int32]),
     "bjx_maximum_eigenvalue": (C.c_int, [C.c_void_p, _f32p, C.c_int64, C.c_int32, _f32p, _f32p]),
     "bjx_permutation_scratch_bytes": (C.c_size_t, [C.c_int64]),

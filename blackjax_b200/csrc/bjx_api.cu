@@ -960,6 +960,41 @@ extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_r
   return rc;
 }
 
+// window_adaptation_low_rank(...).run, run natively: the loop of bjx_adapt_shared_run with bjx_lowrank_window_update as
+// the per-step update.  schedule[t] = stage | window_end << 1 | retained << 2.  Nothing in the loop waits for the device.
+extern "C" int bjx_lowrank_window_run(bjx_handle_t h, const uint32_t* rng_key, const uint8_t* schedule, int32_t num_steps,
+                                      float* q, float* logp, float* grad, float* state, float* step_size_chain,
+                                      float target_acceptance, float gamma, float cutoff, int32_t max_num_doublings,
+                                      int32_t num_integration_steps, float* eps_history, float* acceptance_scratch,
+                                      int32_t* steps_scratch, unsigned long long* leapfrog_counter) {
+  if (!h || !rng_key || !schedule || !q || !logp || !grad || !state || !step_size_chain || !acceptance_scratch || num_steps < 0)
+    return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  if ((max_num_doublings > 0) == (num_integration_steps > 0))
+    return bjx_fail(h, BJX_E_INVALID, "give max_num_doublings (NUTS) or num_integration_steps (HMC)");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  if (num_steps == 0) return 0;
+  int rc = split_step_keys(h, rng_key, num_steps);
+  if (rc) return rc;
+  SharedStepKeys shared(h);
+  for (int t = 0; t < num_steps && rc == 0; ++t) {
+    bjx_info info{};
+    info.acceptance_rate = acceptance_scratch;
+    info.num_integration_steps = (leapfrog_counter && steps_scratch) ? steps_scratch : nullptr;
+    const uint32_t* key_t = h->sample_keys + 2 * (size_t)t;
+    rc = max_num_doublings > 0
+             ? bjx_nuts_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, max_num_doublings, &info, nullptr, nullptr)
+             : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, num_integration_steps, &info);
+    if (rc == 0 && info.num_integration_steps) {
+      k_accum_steps<<<sm_count(), 256, 0, h->stream>>>(h->cfg.n_chains, steps_scratch, leapfrog_counter);
+      BJX_CHECK_LAUNCH("k_accum_steps");
+    }
+    if (rc == 0)
+      rc = bjx_lowrank_window_update(h, state, q, grad, acceptance_scratch, schedule[t], target_acceptance, gamma, cutoff,
+                                     step_size_chain, eps_history);
+  }
+  return rc;
+}
+
 // ---- PRNG ----------------------------------------------------------------------------------------------
 // h may be NULL: the call then runs on the calling thread's registered stream (bjx_set_default_stream; the legacy
 // default stream until one is registered).

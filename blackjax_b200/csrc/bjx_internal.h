@@ -71,3 +71,6 @@ int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps);
 int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q);
 // bjx_mclmc.cu: dim >= 2, a diagonal metric and the row kernels, or BJX_E_UNSUPPORTED with "<name> ..." as the reason
 int mclmc_transition_supported(bjx_handle_t h, const char* name);
+// bjx_meads.cu, shared with the low-rank window adaptation (bjx_lowrank_window.cu): the install of (sigma, U, lam) into a
+// rank-k low-rank metric block (k_lrd_install).
+void launch_lrd_install(int D, int k, const float* sigma, const float* U, const float* lam, float* blk, cudaStream_t s);

@@ -513,6 +513,43 @@ int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, const
 /* final step size exp(log_step_avg) (staged_adaptation.py:303) into step_size_out [1] (device) */
 int bjx_adapt_shared_final(bjx_handle_t h, const float* state, float* step_size_out);
 
+/* ---- Low-rank window adaptation (low_rank_adaptation.py:458-652, buffer_policy="reset"), pooled over chains ----------
+ * ONE step size and ONE low-rank metric M^-1 = diag(sigma) (I + U (diag(lam) - I) U^T) diag(sigma) for all C chains of one
+ * GPU, adapted by Stan's window schedule with the Fisher-divergence estimator (_compute_low_rank_metric,
+ * metric_estimators.py:618-808) at every window end.  The handle must hold a rank-k low-rank metric (k = max_rank,
+ * bjx_set_metric_low_rank); the warm-up rewrites its block in place on the stream.  Built for dim <= 512 and 1 <= k <= 16
+ * on the warp kernels; otherwise BJX_E_UNSUPPORTED.
+ * state float32 [bjx_lowrank_window_state_floats(C, D, k)]; its first 64 floats are
+ *   [0..7] the dual-averaging slots of bjx_adapt_shared_* ([5] the current step size, [7] steps taken)
+ *   [8] slow steps of the current window   [9] windows ended
+ *   [32..48) and [48..64) the eigensolver headers of the draws' and the gradients' top-k solves, slots as in
+ *   bjx_meads_lrd_state_floats ([1] iterations of the last solve, [2] its largest relative residual, [3] sticky
+ *   non-converged flag, [4] sum and [5] maximum of the iterations, [6] solves)
+ * followed by sigma[D] | U[D,k] | lam[k] | mu*[D], the metric of the last window end (initially ones, zeros, ones, zeros).
+ * bjx_lowrank_window_init: zero-fills the state, initialises dual averaging at initial_step_size (step_size_chain_out [C]
+ * filled with it) and installs the initial metric.
+ * bjx_lowrank_window_update: one warm-up step after the transition.  schedule = stage | window_end << 1 | retained << 2:
+ * dual averaging on the mean of acceptance_rate [C] every step; on a retained slow step q and grad [C, D] are folded into
+ * the windowed accumulators of the draws and the gradients; every slow step counts towards the window's n = C x steps;
+ * at a window end (a retained slow step) the estimator runs with gamma and cutoff, the metric is re-installed, the
+ * accumulators are reset and dual averaging restarts at exp(log_step_avg).  Retain the last min(steps, B) steps of every
+ * window to reproduce the reference's circular buffer of B steps.  eps_history (nullable, device): step size of step t.
+ * bjx_lowrank_window_run: the whole warm-up as one call, the loop of bjx_adapt_shared_run with this update.
+ * bjx_lowrank_window_final: step_size_out [1] = exp(log_step_avg), mu_star_out [D], sigma_out [D], U_out [D,k],
+ * lam_out [k] (device).  Every reduction has a fixed order: two runs are bit-identical. */
+size_t bjx_lowrank_window_state_floats(int32_t n_chains, int32_t dim, int32_t rank);
+int bjx_lowrank_window_init(bjx_handle_t h, float* state, float initial_step_size, float* step_size_chain_out);
+int bjx_lowrank_window_update(bjx_handle_t h, float* state, const float* q, const float* grad, const float* acceptance_rate,
+                              int32_t schedule, float target_acceptance, float gamma, float cutoff, float* step_size_chain,
+                              float* eps_history);
+int bjx_lowrank_window_run(bjx_handle_t h, const uint32_t* rng_key, const uint8_t* schedule, int32_t num_steps, float* q,
+                           float* logp, float* grad, float* state, float* step_size_chain, float target_acceptance,
+                           float gamma, float cutoff, int32_t max_num_doublings, int32_t num_integration_steps,
+                           float* eps_history, float* acceptance_scratch, int32_t* steps_scratch,
+                           unsigned long long* leapfrog_counter);
+int bjx_lowrank_window_final(bjx_handle_t h, const float* state, float* step_size_out, float* mu_star_out, float* sigma_out,
+                             float* U_out, float* lam_out);
+
 /* ---- ChEES-HMC warm-up (blackjax/adaptation/chees_adaptation.py, mass_matrix_estimation=None; SURVEY 8f item 4) --------------
  * Cross-chain adaptation of the step size (dual averaging on the harmonic mean of the acceptance probabilities) and of the
  * trajectory length (Adam on log T along the ChEES gradient), device resident, two all-gathers of block statistics per
