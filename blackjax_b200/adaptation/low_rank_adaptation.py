@@ -18,7 +18,7 @@ import torch
 from .._lib import check, lib, ptr
 from ..base import AdaptationAlgorithm, AdaptationResults
 from ..mcmc.metrics import LowRankMetric
-from .window_adaptation import build_schedule
+from .window_adaptation import build_schedule, native_run_inputs
 
 __all__ = ["LowRankWindowInfo", "build_growing_window_schedule", "window_adaptation_low_rank"]
 
@@ -189,17 +189,12 @@ def window_adaptation_low_rank(algorithm, logdensity_fn, max_rank: int = 10, ini
         dev = position.device
         sched = schedule_bytes(schedule_fn(num_steps), num_steps)
         state = algorithm.init(position, logdensity_fn)
-        mnd = int(extra_parameters.get("max_num_doublings", 10)) if is_nuts else 0
-        nis = 0 if is_nuts else int(extra_parameters["num_integration_steps"])
-        eng = get_engine(position, logdensity_fn, max_tree_depth=max(10, mnd))
+        eng = get_engine(position, logdensity_fn, max_tree_depth=max(10, int(extra_parameters.get("max_num_doublings", 10))))
         lw = _LowRankWindow(eng, k)
         lw.install(initial_step_size)
         eps_hist = torch.empty(num_steps, dtype=torch.float32, device=dev)
-        q, lp, g = state.position.clone(), state.logdensity.clone(), state.logdensity_grad.clone()
-        acc_scratch = torch.empty(C, dtype=torch.float32, device=dev)
-        steps_scratch = torch.empty(C, dtype=torch.int32, device=dev) if _leapfrog_counter is not None else None
-        rk = rng_key.to(dev).contiguous()
-        eng._key_mode(rk, 0)
+        mnd, nis, q, lp, g, acc_scratch, steps_scratch, rk = native_run_inputs(eng, state, rng_key, 0, is_nuts,
+                                                                                extra_parameters, _leapfrog_counter)
         check(lib().bjx_lowrank_window_run(eng.h, ptr(rk), sched, int(num_steps), ptr(q), ptr(lp), ptr(g), ptr(lw.state),
                                            ptr(lw.eps_c), float(target_acceptance_rate), float(gamma), float(cutoff), mnd,
                                            nis, ptr(eps_hist), ptr(acc_scratch), ptr(steps_scratch),

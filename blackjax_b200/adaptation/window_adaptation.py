@@ -124,6 +124,22 @@ def _allgather_stats(block, group):
     return out.view((world,) + tuple(block.shape))
 
 
+def native_run_inputs(eng, state, rng_key, chain_offset, is_nuts, extra_parameters, leapfrog_counter):
+    """What the native warm-up loops (bjx_adapt_shared_run, bjx_lowrank_window_run) take besides their recipe's state:
+    ``(max_num_doublings, num_integration_steps, q, logp, grad, acceptance_scratch, steps_scratch, rng_key)`` -- the
+    transition's length argument with the other one 0, clones of ``state`` that the loop advances in place, the
+    per-chain scratch arrays (the leapfrog counts only when they are accumulated) and the contiguous device key, which
+    the engine is told is one step key shared by the chains from global index ``chain_offset``."""
+    mnd = int(extra_parameters.get("max_num_doublings", 10)) if is_nuts else 0
+    nis = 0 if is_nuts else int(extra_parameters["num_integration_steps"])
+    q, lp, g = state.position.clone(), state.logdensity.clone(), state.logdensity_grad.clone()
+    acc_scratch = torch.empty(eng.C, dtype=torch.float32, device=eng.device)
+    steps_scratch = torch.empty(eng.C, dtype=torch.int32, device=eng.device) if leapfrog_counter is not None else None
+    rk = rng_key.to(eng.device).contiguous()
+    eng._key_mode(rk, chain_offset)
+    return mnd, nis, q, lp, g, acc_scratch, steps_scratch, rk
+
+
 def window_adaptation(algorithm, logdensity_fn, is_mass_matrix_diagonal: bool = True,
                       initial_step_size: float = 1.0, target_acceptance_rate: float = 0.80, shared: bool = False,
                       process_group=None, **extra_parameters):
@@ -145,16 +161,11 @@ def window_adaptation(algorithm, logdensity_fn, is_mass_matrix_diagonal: bool = 
         world, rank = 1, 0
         if shared and dist.is_available() and dist.is_initialized():
             world, rank = dist.get_world_size(process_group), dist.get_rank(process_group)
-        # shared mode: one step key per warm-up step; chain c of this rank uses split(step_key, C_global)[rank*C + c]
-        # (staged_adaptation.py:920), derived inside the transition kernel
-        mcmc_kernel = algorithm.build_kernel(chain_offset=rank * C)
         if shared and not dense and position.is_cuda:
             # ---- device-resident shared adaptation (libbjx bjx_adapt_shared_*): block statistics, ONE NCCL all-gather,
             # merge + dual averaging + window bookkeeping on the device; no host round trip per warm-up step --------
             from .._comm import nccl_comm
             comm, n_ranks, rank = nccl_comm(dev, process_group)
-            mcmc_kernel = algorithm.build_kernel(chain_offset=rank * C)
-            step_keys = bjx_random.split(rng_key.to(dev), num_steps)
             L = lib()
             st = torch.empty(L.bjx_adapt_shared_state_floats(C, D, n_ranks), dtype=torch.float32, device=dev)
             eps_c = torch.empty(C, dtype=torch.float32, device=dev)
@@ -163,16 +174,12 @@ def window_adaptation(algorithm, logdensity_fn, is_mass_matrix_diagonal: bool = 
             check(L.bjx_adapt_shared_init(eng.h, ptr(st), float(initial_step_size), ptr(eps_c), ptr(imm)), eng.h)
             eng._imm, eng._imm_key = imm, (imm.data_ptr(), tuple(imm.shape), imm._version, str(imm.device))
             # the loop itself runs in libbjx (bjx_adapt_shared_run): transition, block statistics, all-gather, device-side
-            # update per warm-up step, nothing waits for the device
-            is_nuts = "num_integration_steps" not in extra_parameters
-            mnd = int(extra_parameters.get("max_num_doublings", 10)) if is_nuts else 0
-            nis = 0 if is_nuts else int(extra_parameters["num_integration_steps"])
+            # update per warm-up step, nothing waits for the device.  Chain c of this rank uses
+            # split(step_key, C_global)[rank * C + c] (staged_adaptation.py:920), derived inside the transition kernel
             sched = bytes(int(stage) | (int(window_end) << 1) for stage, window_end in schedule)
-            q, lp, g = state.position.clone(), state.logdensity.clone(), state.logdensity_grad.clone()
-            acc_scratch = torch.empty(C, dtype=torch.float32, device=dev)
-            steps_scratch = torch.empty(C, dtype=torch.int32, device=dev) if _leapfrog_counter is not None else None
-            eng._key_mode(rng_key.to(dev).contiguous(), rank * C)
-            rk = rng_key.to(dev).contiguous()
+            mnd, nis, q, lp, g, acc_scratch, steps_scratch, rk = native_run_inputs(
+                eng, state, rng_key, rank * C, "num_integration_steps" not in extra_parameters, extra_parameters,
+                _leapfrog_counter)
             check(L.bjx_adapt_shared_run(eng.h, comm, n_ranks, ptr(rk), sched, int(num_steps), ptr(q), ptr(lp), ptr(g), ptr(st),
                                          ptr(eps_c), ptr(imm), float(target_acceptance_rate), mnd, nis, ptr(eps_hist),
                                          ptr(acc_scratch), ptr(steps_scratch), ptr(_leapfrog_counter)), eng.h)
@@ -183,6 +190,9 @@ def window_adaptation(algorithm, logdensity_fn, is_mass_matrix_diagonal: bool = 
             step_size = float(step.item())   # the one host read of the warm-up
             parameters = {"step_size": step_size, "inverse_mass_matrix": imm, **extra_parameters}
             return AdaptationResults(state, parameters), eps_hist.cpu()
+        # shared mode: one step key per warm-up step; chain c of this rank uses split(step_key, C_global)[rank*C + c]
+        # (staged_adaptation.py:920), derived inside the transition kernel
+        mcmc_kernel = algorithm.build_kernel(chain_offset=rank * C)
         if shared:
             step_keys = bjx_random.split(rng_key.to(dev), num_steps)
             da = _da_init(initial_step_size)

@@ -24,11 +24,12 @@
 
 #include "bjx_handle.h"
 #include "bjx_internal.h"
+#include "bjx_pooled_step.cuh"
 
 namespace bjx {
 
 constexpr int kStatBlock = BJX_STAT_BLOCK_CHAINS;
-constexpr int kHdr = 16;  // scalar slots at the head of the adaptation state
+constexpr int kHdr = 16;  // scalar slots at the head of the adaptation state: PS_* (bjx_pooled_step.cuh), the rest unused
 
 // ---- per-block chain-pooled statistics ------------------------------------------------------------------------
 // grid (ceil(D/32), n_blocks), block (32, 8): block (bx, by) reduces columns [32 bx, +32) over chains [by*B, (by+1)*B)
@@ -86,26 +87,12 @@ __global__ void k_block_stats(int C, int D, const float* __restrict__ x, const f
 }
 
 // ---- merge + dual averaging + window bookkeeping: one CTA ---------------------------------------------------------
-// state: [0] log_step [1] log_step_avg [2] step [3] avg_error [4] mu [5] eps [6] w_n [7] t; [16, 16+D) w_mean; [16+D, 16+2D) w_m2
-struct MergeScalars {
-  float n, acc;
-};
-__device__ __forceinline__ void cgl_factors(float na, float nb, float& f_mean, float& f_cross, float& n_ab) {
-  // metric_buffers.py:334-393 with the reference's scalar arithmetic (exact integer counts, one rounding to float32)
-  const double ab = (double)na + (double)nb;
-  n_ab = (float)ab;
-  f_mean = (float)((double)nb / ab);
-  f_cross = (float)((double)na * (double)nb / ab);
-}
-
+// state: header | w_mean [D] | w_m2 [D] (the window accumulator, its count in PS_WINDOW_N) | block records
 __global__ void k_shared_adapt(int D, int nblk, const float* __restrict__ blocks, float* __restrict__ st, int stage, int window_end,
                                float target, float* __restrict__ imm, float* __restrict__ eps_hist) {
   const int S = 2 + 2 * D;
-  // every thread replays the scalar recurrences (identical results), threads own dimensions
-  float n = blocks[1], acc = blocks[0];
-  const float w_n0 = st[6];
-  float wn_new = w_n0, f_mean_w = 0.f, f_cross_w = 0.f;
-  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+  const float w_n0 = st[PS_WINDOW_N];
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {  // threads own dimensions; each replays the scalar count recurrence
     float nn = blocks[1];
     float mean = blocks[2 + d], m2 = blocks[2 + D + d];
     for (int b = 1; b < nblk; ++b) {
@@ -135,38 +122,14 @@ __global__ void k_shared_adapt(int D, int nblk, const float* __restrict__ blocks
       }
     }
   }
-  for (int b = 1; b < nblk; ++b) {
-    const float* g = blocks + (size_t)b * S;
-    float fm, fc, nab;
-    cgl_factors(n, g[1], fm, fc, nab);
-    n = nab;
-    acc += g[0];
-  }
-  if (stage == 1) {
-    cgl_factors(w_n0, n, f_mean_w, f_cross_w, wn_new);
-    if (window_end) wn_new = 0.f;
-  }
-  __syncthreads();  // every thread has read the scalar slots
+  __syncthreads();  // every thread has read the window count
   if (threadIdx.x == 0) {
-    // dual averaging on the mean acceptance rate of all chains (dual_averaging.py:101-123; staged_adaptation.py:153-171)
-    float log_step = st[0], avg_log_step = st[1], step = st[2], avg_error = st[3], mu = st[4];
-    const float gradient = target - acc / n;
-    const float reg_step = step + 10.f;
-    const float eta_t = powf(step, -0.75f);
-    avg_error = (1.f - (1.f / reg_step)) * avg_error + gradient / reg_step;
-    const float log_x = mu - (sqrtf(step) / 0.05f) * avg_error;
-    const float log_x_avg = eta_t * log_step + (1.f - eta_t) * avg_log_step;
-    log_step = log_x; avg_log_step = log_x_avg; step = step + 1.f;
-    if (window_end) {  // staged_adaptation.py:233-249
-      const float x = expf(avg_log_step);
-      log_step = logf(x); avg_log_step = 0.f; step = 1.f; avg_error = 0.f; mu = logf(10.f * x);
+    const float n = pooled_step_size_update(nblk, blocks, S, st, window_end, target, eps_hist);
+    if (stage == 1) {
+      float fm, fc, wn_new;
+      cgl_factors(w_n0, n, fm, fc, wn_new);
+      st[PS_WINDOW_N] = window_end ? 0.f : wn_new;
     }
-    const float eps = expf(log_step);
-    st[0] = log_step; st[1] = avg_log_step; st[2] = step; st[3] = avg_error; st[4] = mu; st[5] = eps;
-    st[6] = wn_new;
-    const int t = (int)st[7];
-    if (eps_hist) eps_hist[t] = eps;
-    st[7] = (float)(t + 1);
   }
 }
 
@@ -174,13 +137,16 @@ __global__ void k_fill_from(int n, const float* __restrict__ src, float* __restr
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = src[0];
 }
+void launch_fill_from(int n, const float* src, float* dst, cudaStream_t s) {
+  k_fill_from<<<(n + 255) / 256, 256, 0, s>>>(n, src, dst);
+}
 __global__ void k_adapt_init(int D, float* st, float eps0, float* imm) {
   for (int d = threadIdx.x; d < 2 * D; d += blockDim.x) st[kHdr + d] = 0.f;
   for (int d = threadIdx.x; d < D; d += blockDim.x) imm[d] = 1.f;
   if (threadIdx.x == 0) {
-    st[0] = logf(eps0); st[1] = 0.f; st[2] = 1.f; st[3] = 0.f; st[4] = logf(10.f * eps0); st[5] = expf(logf(eps0));
-    st[6] = 0.f; st[7] = 0.f;
-    for (int k = 8; k < kHdr; ++k) st[k] = 0.f;
+    da_init(st + PS_DA, eps0);
+    st[PS_EPS] = da_step_size(st + PS_DA);
+    for (int k = PS_WINDOW_N; k < kHdr; ++k) st[k] = 0.f;
   }
 }
 
@@ -268,12 +234,10 @@ extern "C" int bjx_allgather_stats(bjx_handle_t h, void* nccl_comm, const float*
   return r == ncclSuccess ? 0 : nccl_fail(h, r, "ncclAllGather");
 }
 
-static inline int n_stat_blocks(int C) { return (C + kStatBlock - 1) / kStatBlock; }
-
 extern "C" int64_t bjx_adapt_shared_state_floats(int32_t n_chains_local, int32_t dim, int32_t n_ranks) {
   if (n_chains_local <= 0 || dim <= 0 || n_ranks <= 0) return 0;
   const int64_t blk = 2 + 2 * (int64_t)dim;
-  return kHdr + 2 * (int64_t)dim + (int64_t)n_stat_blocks(n_chains_local) * blk * (1 + n_ranks);
+  return kHdr + 2 * (int64_t)dim + (int64_t)cov_stat_blocks(n_chains_local) * blk * (1 + n_ranks);
 }
 
 extern "C" int bjx_adapt_shared_init(bjx_handle_t h, float* state, float initial_step_size, float* step_size_chain_out, float* imm_out) {
@@ -283,7 +247,7 @@ extern "C" int bjx_adapt_shared_init(bjx_handle_t h, float* state, float initial
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   k_adapt_init<<<1, 256, 0, h->stream>>>(D, state, initial_step_size, imm_out);
   BJX_CHECK_LAUNCH("k_adapt_init");
-  k_fill_from<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + 5, step_size_chain_out);
+  launch_fill_from(C, state + PS_EPS, step_size_chain_out, h->stream);
   BJX_CHECK_LAUNCH("k_fill_from");
   return bjx_set_metric(h, BJX_METRIC_DIAG, imm_out);
 }
@@ -296,7 +260,7 @@ extern "C" int bjx_adapt_shared_update(bjx_handle_t h, void* nccl_comm, int32_t 
   if (window_end && stage != 1) return bjx_fail(h, BJX_E_INVALID, "a window ends on a slow-stage step");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   const int C = h->cfg.n_chains, D = h->cfg.dim;
-  const int nb = n_stat_blocks(C);
+  const int nb = cov_stat_blocks(C);
   const size_t blk = 2 + 2 * (size_t)D;
   float* local = state + kHdr + 2 * (size_t)D;
   float* gathered = local + (size_t)nb * blk;
@@ -310,7 +274,7 @@ extern "C" int bjx_adapt_shared_update(bjx_handle_t h, void* nccl_comm, int32_t 
   }
   k_shared_adapt<<<1, 512, 0, h->stream>>>(D, nb * n_ranks, merged_in, state, stage, window_end, target_acceptance, imm, eps_history);
   BJX_CHECK_LAUNCH("k_shared_adapt");
-  k_fill_from<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + 5, step_size_chain);
+  launch_fill_from(C, state + PS_EPS, step_size_chain, h->stream);
   BJX_CHECK_LAUNCH("k_fill_from");
   if (window_end) return bjx_set_metric(h, BJX_METRIC_DIAG, imm);  // mass_matrix_sqrt of the new metric, on the stream
   return 0;
@@ -543,17 +507,14 @@ __global__ void k_chees_finish(int nblk, const float* __restrict__ blocks2, floa
   // step size: dual averaging on target - harmonic mean of the non-divergent acceptance probabilities
   float hm = 1.0f / (st[CH_HM_SUM] / st[CH_HM_N]);
   if (!isfinite(hm)) hm = 0.f;
-  float log_x = st[CH_DA_LOGX], log_x_avg = st[CH_DA_LOGX_AVG], da_step = st[CH_DA_STEP], err = st[CH_DA_ERR];
-  const float mu = st[CH_DA_MU];
-  {
-    const float gradient = target - hm;
-    const float reg_step = da_step + 10.f;
-    const float eta_t = powf(da_step, -0.75f);
-    const float nerr = (1.f - (1.f / reg_step)) * err + gradient / reg_step;
-    const float nlog_x = mu - (sqrtf(da_step) / 0.05f) * nerr;
-    const float navg = eta_t * log_x + (1.f - eta_t) * log_x_avg;
-    const float neps = expf(nlog_x);
-    if (isfinite(neps)) { eps = neps; log_x = nlog_x; log_x_avg = navg; da_step += 1.f; err = nerr; }
+  float da[5];  // CH_DA_LOGX .. CH_DA_MU are a dual-averaging state; the update is kept only when the new step size is finite
+  for (int k = 0; k < 5; ++k) da[k] = st[CH_DA_LOGX + k];
+  float log_x = da[0];
+  da_update_step(da, hm, target);
+  if (isfinite(da_step_size(da))) {
+    eps = da_step_size(da);
+    log_x = da[0];
+    for (int k = 0; k < 4; ++k) st[CH_DA_LOGX + k] = da[k];
   }
   const float uw = powf(step, -decay);
   const float log_eps_ma = (1.f - uw) * st[CH_LOG_EPS_MA] + uw * log_x;
@@ -580,7 +541,6 @@ __global__ void k_chees_finish(int nblk, const float* __restrict__ blocks2, floa
   float newT = expf(log_T_ma);
   newT = fminf(fmaxf(newT, eps), max_leapfrog * eps);
   st[CH_EPS] = eps; st[CH_LOG_EPS_MA] = log_eps_ma; st[CH_T] = newT; st[CH_LOG_T_MA] = log_T_ma;
-  st[CH_DA_LOGX] = log_x; st[CH_DA_LOGX_AVG] = log_x_avg; st[CH_DA_STEP] = da_step; st[CH_DA_ERR] = err;
   st[CH_RGA] = (float)(rga + 1);
   st[CH_STEP] = step + 1.f;
   st[CH_GRAD] = grad;
@@ -602,7 +562,7 @@ __global__ void k_chees_init(float* st, float eps0, int max_bits, float jitter_a
   if (threadIdx.x != 0) return;
   for (int k = 0; k < kChHdr; ++k) st[k] = 0.f;
   st[CH_EPS] = eps0; st[CH_T] = eps0;
-  st[CH_DA_LOGX] = logf(eps0); st[CH_DA_STEP] = 1.f; st[CH_DA_MU] = logf(10.f * eps0);
+  da_init(st + CH_DA_LOGX, eps0);
   st[CH_STEP] = 1.f; st[CH_MAX_BITS] = (float)max_bits; st[CH_JITTER_AMOUNT] = jitter_amount;
   const float j0 = halton_f(0, max_bits) * jitter_amount + (1.f - jitter_amount);
   st[CH_L] = ceilf(j0 * (eps0 / eps0));
@@ -812,13 +772,13 @@ __global__ void k_mm_init(int D, float* __restrict__ ms, float c_global, float t
 }
 
 // The launchers of the block statistics and the block covariance accumulators, shared by ChEES and MEADS-LRD (bjx_meads.cu).
-int cov_stat_blocks(int C) { return n_stat_blocks(C); }
+int cov_stat_blocks(int C) { return (C + kStatBlock - 1) / kStatBlock; }
 size_t cov_block_floats(int D) { return 2 + (size_t)D + (size_t)D * D; }
 void launch_block_stats(int C, int D, const float* x, const float* acc, float* out, cudaStream_t s) {
-  k_block_stats<<<dim3((D + 31) / 32, n_stat_blocks(C)), dim3(32, 8), 0, s>>>(C, D, x, acc, out);
+  k_block_stats<<<dim3((D + 31) / 32, cov_stat_blocks(C)), dim3(32, 8), 0, s>>>(C, D, x, acc, out);
 }
 void launch_cov_fold(int C, int D, const float* q, const float* stats, float* cov, cudaStream_t s) {
-  const int nb = n_stat_blocks(C), tiles = (D + kSyT - 1) / kSyT;
+  const int nb = cov_stat_blocks(C), tiles = (D + kSyT - 1) / kSyT;
   const size_t sstride = 2 + 2 * (size_t)D;
   k_cov_syrk<<<dim3(tiles * (tiles + 1) / 2, nb), 256, 0, s>>>(C, D, q, stats, sstride, cov, cov_block_floats(D));
   k_cov_mean_update<<<nb, 256, 0, s>>>(C, D, stats, sstride, cov, cov_block_floats(D));
@@ -847,7 +807,7 @@ struct ChLayout {
 };
 ChLayout ch_layout(int C, int D, int n_ranks) {
   ChLayout L{};
-  L.nb = n_stat_blocks(C);
+  L.nb = cov_stat_blocks(C);
   L.S1 = 3 + 3 * (size_t)D;
   size_t o = kChHdr + 2 * (size_t)D;
   L.w = o; o += C;
@@ -870,7 +830,7 @@ MmLayout mm_layout(int C, int D, int n_ranks, int options) {
   MmLayout L{};
   const size_t d = (size_t)D;
   const bool fl = options & BJX_CHEES_LENGTH_FLOOR;
-  L.nb = n_stat_blocks(C);
+  L.nb = cov_stat_blocks(C);
   L.S1 = 3 + 3 * d;
   L.Sm = 2 + 2 * d;
   L.R = (size_t)L.nb * (L.S1 + L.Sm);
@@ -986,7 +946,7 @@ int chees_step(bjx_handle_t h, void* comm, int n_ranks, int options, float* stat
   }
   k_chees_finish<<<1, 32, 0, s>>>(nb * n_ranks, m2, state, lr, b1, b2, target, decay, (float)max_lf, hist, ms, lam_hist,
                                   eng_hist);
-  k_fill_from<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_EPS, eps_c);
+  launch_fill_from(C, state + CH_EPS, eps_c, s);
   k_fill_steps<<<(C + 255) / 256, 256, 0, s>>>(C, state + CH_L, steps_c);
   BJX_CHECK_LAUNCH("k_chees_finish");
   if (in_window) return bjx_set_metric(h, BJX_METRIC_DIAG, imm);  // mass_matrix_sqrt of the new estimate, on the stream
@@ -1041,7 +1001,7 @@ extern "C" int bjx_chees_init(bjx_handle_t h, float* state, float step_size, int
   const int C = h->cfg.n_chains;
   k_chees_init<<<1, 32, 0, h->stream>>>(state, step_size, max_bits, jitter_amount);
   BJX_CHECK_LAUNCH("k_chees_init");
-  k_fill_from<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + CH_EPS, step_size_chain_out);
+  launch_fill_from(C, state + CH_EPS, step_size_chain_out, h->stream);
   k_fill_steps<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + CH_L, steps_chain_out);
   BJX_CHECK_LAUNCH("k_fill");
   return 0;

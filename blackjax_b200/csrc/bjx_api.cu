@@ -923,16 +923,15 @@ static __global__ void k_accum_steps(int C, const int* __restrict__ n, unsigned 
   if ((threadIdx.x & 31) == 0 && a) atomicAdd(out, a);
 }
 
-// window_adaptation(...).run for the shared (one step size, one diagonal metric) recipe, run natively
-// (staged_adaptation.py:906-966): per warm-up step one transition (NUTS: max_num_doublings > 0, HMC: num_integration_steps
-// > 0) with split(rng_key, num_steps)[t] as the step key, then bjx_adapt_shared_update.  schedule[t] = stage | (window_end
-// << 1) (staged_adaptation.py:315-405).  Nothing in the loop waits for the device.
-extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, const uint32_t* rng_key,
-                                    const uint8_t* schedule, int32_t num_steps, float* q, float* logp, float* grad,
-                                    float* state, float* step_size_chain, float* imm, float target_acceptance,
-                                    int32_t max_num_doublings, int32_t num_integration_steps, float* eps_history,
-                                    float* acceptance_scratch, int32_t* steps_scratch, unsigned long long* leapfrog_counter) {
-  if (!h || !rng_key || !schedule || !q || !logp || !grad || !state || !step_size_chain || !imm || !acceptance_scratch || num_steps < 0)
+// The native loop of the pooled window recipes (staged_adaptation.py:906-966): per warm-up step one transition (NUTS:
+// max_num_doublings > 0, HMC: num_integration_steps > 0) with split(rng_key, num_steps)[t] as the step key and
+// step_size_chain as the step sizes, then update(t), the recipe's adaptation on the new (q, grad, acceptance_scratch).
+// Nothing in the loop waits for the device.
+template <class Update>
+static int warmup_run(bjx_handle_t h, const uint32_t* rng_key, int32_t num_steps, float* q, float* logp, float* grad,
+                      float* step_size_chain, int32_t max_num_doublings, int32_t num_integration_steps,
+                      float* acceptance_scratch, int32_t* steps_scratch, unsigned long long* leapfrog_counter, Update update) {
+  if (!h || !rng_key || !q || !logp || !grad || !step_size_chain || !acceptance_scratch || num_steps < 0)
     return bjx_fail(h, BJX_E_INVALID, "bad argument");
   if ((max_num_doublings > 0) == (num_integration_steps > 0))
     return bjx_fail(h, BJX_E_INVALID, "give max_num_doublings (NUTS) or num_integration_steps (HMC)");
@@ -953,46 +952,38 @@ extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_r
       k_accum_steps<<<sm_count(), 256, 0, h->stream>>>(h->cfg.n_chains, steps_scratch, leapfrog_counter);
       BJX_CHECK_LAUNCH("k_accum_steps");
     }
-    if (rc == 0)
-      rc = bjx_adapt_shared_update(h, nccl_comm, n_ranks, state, q, acceptance_scratch, schedule[t] & 1, (schedule[t] >> 1) & 1,
-                                   target_acceptance, step_size_chain, imm, eps_history);
+    if (rc == 0) rc = update(t);
   }
   return rc;
 }
 
-// window_adaptation_low_rank(...).run, run natively: the loop of bjx_adapt_shared_run with bjx_lowrank_window_update as
-// the per-step update.  schedule[t] = stage | window_end << 1 | retained << 2.  Nothing in the loop waits for the device.
+// window_adaptation(...).run for the shared (one step size, one diagonal metric) recipe: schedule[t] = stage |
+// window_end << 1 (staged_adaptation.py:315-405)
+extern "C" int bjx_adapt_shared_run(bjx_handle_t h, void* nccl_comm, int32_t n_ranks, const uint32_t* rng_key,
+                                    const uint8_t* schedule, int32_t num_steps, float* q, float* logp, float* grad,
+                                    float* state, float* step_size_chain, float* imm, float target_acceptance,
+                                    int32_t max_num_doublings, int32_t num_integration_steps, float* eps_history,
+                                    float* acceptance_scratch, int32_t* steps_scratch, unsigned long long* leapfrog_counter) {
+  if (!schedule || !state || !imm) return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  return warmup_run(h, rng_key, num_steps, q, logp, grad, step_size_chain, max_num_doublings, num_integration_steps,
+                    acceptance_scratch, steps_scratch, leapfrog_counter, [&](int t) {
+                      return bjx_adapt_shared_update(h, nccl_comm, n_ranks, state, q, acceptance_scratch, schedule[t] & 1,
+                                                     (schedule[t] >> 1) & 1, target_acceptance, step_size_chain, imm, eps_history);
+                    });
+}
+
+// window_adaptation_low_rank(...).run: schedule[t] = stage | window_end << 1 | retained << 2
 extern "C" int bjx_lowrank_window_run(bjx_handle_t h, const uint32_t* rng_key, const uint8_t* schedule, int32_t num_steps,
                                       float* q, float* logp, float* grad, float* state, float* step_size_chain,
                                       float target_acceptance, float gamma, float cutoff, int32_t max_num_doublings,
                                       int32_t num_integration_steps, float* eps_history, float* acceptance_scratch,
                                       int32_t* steps_scratch, unsigned long long* leapfrog_counter) {
-  if (!h || !rng_key || !schedule || !q || !logp || !grad || !state || !step_size_chain || !acceptance_scratch || num_steps < 0)
-    return bjx_fail(h, BJX_E_INVALID, "bad argument");
-  if ((max_num_doublings > 0) == (num_integration_steps > 0))
-    return bjx_fail(h, BJX_E_INVALID, "give max_num_doublings (NUTS) or num_integration_steps (HMC)");
-  BJX_CUDA(cudaSetDevice(h->cfg.device));
-  if (num_steps == 0) return 0;
-  int rc = split_step_keys(h, rng_key, num_steps);
-  if (rc) return rc;
-  SharedStepKeys shared(h);
-  for (int t = 0; t < num_steps && rc == 0; ++t) {
-    bjx_info info{};
-    info.acceptance_rate = acceptance_scratch;
-    info.num_integration_steps = (leapfrog_counter && steps_scratch) ? steps_scratch : nullptr;
-    const uint32_t* key_t = h->sample_keys + 2 * (size_t)t;
-    rc = max_num_doublings > 0
-             ? bjx_nuts_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, max_num_doublings, &info, nullptr, nullptr)
-             : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, num_integration_steps, &info);
-    if (rc == 0 && info.num_integration_steps) {
-      k_accum_steps<<<sm_count(), 256, 0, h->stream>>>(h->cfg.n_chains, steps_scratch, leapfrog_counter);
-      BJX_CHECK_LAUNCH("k_accum_steps");
-    }
-    if (rc == 0)
-      rc = bjx_lowrank_window_update(h, state, q, grad, acceptance_scratch, schedule[t], target_acceptance, gamma, cutoff,
-                                     step_size_chain, eps_history);
-  }
-  return rc;
+  if (!schedule || !state) return bjx_fail(h, BJX_E_INVALID, "bad argument");
+  return warmup_run(h, rng_key, num_steps, q, logp, grad, step_size_chain, max_num_doublings, num_integration_steps,
+                    acceptance_scratch, steps_scratch, leapfrog_counter, [&](int t) {
+                      return bjx_lowrank_window_update(h, state, q, grad, acceptance_scratch, schedule[t], target_acceptance,
+                                                       gamma, cutoff, step_size_chain, eps_history);
+                    });
 }
 
 // ---- PRNG ----------------------------------------------------------------------------------------------

@@ -15,7 +15,11 @@ void launch_prng_split(const uint32_t* keys, long long n, int num, uint32_t* out
 void launch_prng_fold_in(const uint32_t* keys, long long n, uint32_t data, uint32_t* out, cudaStream_t s);
 void launch_prng_draw(int mode, const uint32_t* keys, long long n, long long per_key, void* out, cudaStream_t s);
 void launch_diag_mass_sqrt(const float* imm, long long n, float* out, cudaStream_t s);
+// per-chain dual averaging on st [C, 5] (bjx_da.cuh): op 0 init from in = eps0 [C], 1 update on in = acceptance [C], 2 restart,
+// 3 final; eps_out [C] (optional for 0-2) takes the step size
 void launch_da(int op, int C, float* st, const float* in, float target, float* eps_out, cudaStream_t s);
+// dst[i] = src[0], i < n: a device scalar broadcast to the per-chain array the transition kernels read
+void launch_fill_from(int n, const float* src, float* dst, cudaStream_t s);
 void launch_welford_update(long long n, const float* x, float* mean, float* m2, int count, cudaStream_t s);
 void launch_welford_final(long long n, float* mean, float* m2, int count, float* imm, cudaStream_t s);
 void launch_welford_dense_update(int C, int D, const float* x, float* mean, float* m2, int count, cudaStream_t s);

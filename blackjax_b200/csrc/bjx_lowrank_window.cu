@@ -3,8 +3,8 @@
 // for all chains of one GPU.
 //
 // Per warm-up step (schedule byte = stage | window_end << 1 | retained << 2):
-//  - dual averaging on the mean acceptance rate of all chains, the float32 arithmetic of k_shared_adapt (bjx_adapt.cu);
-//    the acceptance sums come from the k_block_stats records of the positions, summed in global block order;
+//  - dual averaging on the mean acceptance rate of all chains (pooled_step_size_update, bjx_pooled_step.cuh), fed by the
+//    k_block_stats records of the positions;
 //  - on a retained slow step the positions and the gradients of all chains are folded into two windowed covariance
 //    accumulators (k_cov_syrk / cgl_update_batch, per statistic block).  The reference keeps a circular buffer of the last
 //    B draws of the window (metric_recipes.py:601-700); the host knows the schedule, so it marks as retained exactly the
@@ -31,19 +31,18 @@
 #include "bjx_handle.h"
 #include "bjx_internal.h"
 #include "bjx_lrd_eig.cuh"
+#include "bjx_pooled_step.cuh"
 
 namespace bjx {
 namespace {
 
-constexpr int kStatBlk = BJX_STAT_BLOCK_CHAINS;
 constexpr int kLwHdr = 64;          // scalar slots | eigensolver header of S_x | eigensolver header of S_a
 constexpr int kLwMaxDim = 512, kLwMaxRank = 16, kQ = 2 * kLwMaxRank;
 constexpr int kJacobiSweepsD = 40;
-// header slots (the first eight are k_shared_adapt's)
-enum { LW_LOG_STEP = 0, LW_LOG_AVG, LW_STEP, LW_ERR, LW_MU, LW_EPS, LW_UNUSED, LW_T, LW_LEN, LW_WINDOWS };
+// header slots after PS_* (bjx_pooled_step.cuh): slow steps of the open window, windows ended
+enum { LW_LEN = 8, LW_WINDOWS };
 constexpr int kEhx = 32, kEha = 48;  // LRD_* slots of the two solves (include/bjx.h)
 
-int stat_blocks(int C) { return (C + kStatBlk - 1) / kStatBlk; }
 size_t even(size_t n) { return (n + 1) & ~(size_t)1; }
 
 size_t lrd_eig_basis_floats(int D, int k) { return (size_t)D * lrd_basis_cols(D, k); }
@@ -60,7 +59,7 @@ LwLayout lw_layout(int C, int D, int k) {
   LwLayout L{};
   const size_t d = (size_t)D, sc = cov_block_floats(D);
   const bool solve = D > 2 * k;
-  L.nb = stat_blocks(C);
+  L.nb = cov_stat_blocks(C);
   L.Sc = sc;
   size_t o = kLwHdr;
   L.sigma = o; o += d;
@@ -88,14 +87,6 @@ LwLayout lw_layout(int C, int D, int k) {
   return L;
 }
 
-// the scalar arithmetic of bjx_adapt.cu's cgl_factors (metric_buffers.py:334-393)
-__device__ __forceinline__ void lw_cgl(float na, float nb, float& f_mean, float& f_cross, float& n_ab) {
-  const double ab = (double)na + (double)nb;
-  n_ab = (float)ab;
-  f_mean = (float)((double)nb / ab);
-  f_cross = (float)((double)na * (double)nb / ab);
-}
-
 __global__ void k_lw_init(int D, int k, float* __restrict__ st, float eps0, const LwLayout L) {
   for (int d = threadIdx.x; d < D; d += blockDim.x) {
     st[L.sigma + d] = 1.f;
@@ -103,48 +94,18 @@ __global__ void k_lw_init(int D, int k, float* __restrict__ st, float eps0, cons
     for (int j = 0; j < k; ++j) st[L.U + (size_t)d * k + j] = 0.f;
   }
   for (int j = threadIdx.x; j < k; j += blockDim.x) st[L.lam + j] = 1.f;
-  if (threadIdx.x == 0) {  // k_adapt_init
-    st[LW_LOG_STEP] = logf(eps0); st[LW_LOG_AVG] = 0.f; st[LW_STEP] = 1.f; st[LW_ERR] = 0.f; st[LW_MU] = logf(10.f * eps0);
-    st[LW_EPS] = expf(logf(eps0));
+  if (threadIdx.x == 0) {
+    da_init(st + PS_DA, eps0);
+    st[PS_EPS] = da_step_size(st + PS_DA);
   }
 }
 
-// dual averaging on the mean acceptance rate (k_shared_adapt's float32 arithmetic) and the window's step count
+// the pooled step-size update and the window's step count
 __global__ void k_lw_adapt(int nblk, const float* __restrict__ blocks, size_t S, float* __restrict__ st, int stage,
                            int window_end, float target, float* __restrict__ eps_hist) {
   if (threadIdx.x != 0) return;
-  float n = blocks[1], acc = blocks[0];
-  for (int b = 1; b < nblk; ++b) {
-    const float* g = blocks + (size_t)b * S;
-    float fm, fc, nab;
-    lw_cgl(n, g[1], fm, fc, nab);
-    n = nab;
-    acc += g[0];
-  }
-  float log_step = st[LW_LOG_STEP], avg_log_step = st[LW_LOG_AVG], step = st[LW_STEP], avg_error = st[LW_ERR], mu = st[LW_MU];
-  const float gradient = target - acc / n;
-  const float reg_step = step + 10.f;
-  const float eta_t = powf(step, -0.75f);
-  avg_error = (1.f - (1.f / reg_step)) * avg_error + gradient / reg_step;
-  const float log_x = mu - (sqrtf(step) / 0.05f) * avg_error;
-  const float log_x_avg = eta_t * log_step + (1.f - eta_t) * avg_log_step;
-  log_step = log_x; avg_log_step = log_x_avg; step = step + 1.f;
-  if (window_end) {
-    const float x = expf(avg_log_step);
-    log_step = logf(x); avg_log_step = 0.f; step = 1.f; avg_error = 0.f; mu = logf(10.f * x);
-  }
-  const float eps = expf(log_step);
-  st[LW_LOG_STEP] = log_step; st[LW_LOG_AVG] = avg_log_step; st[LW_STEP] = step; st[LW_ERR] = avg_error; st[LW_MU] = mu;
-  st[LW_EPS] = eps;
+  pooled_step_size_update(nblk, blocks, S, st, window_end, target, eps_hist);
   if (stage) st[LW_LEN] += 1.f;
-  const int t = (int)st[LW_T];
-  if (eps_hist) eps_hist[t] = eps;
-  st[LW_T] = (float)(t + 1);
-}
-
-__global__ void k_lw_fill(int n, const float* __restrict__ src, float* __restrict__ dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = src[0];
 }
 
 // grid (ceil(D / 256), D, 2): the block accumulators of x (z = 0) or g (z = 1) merged in global block order; raw M2, both
@@ -161,7 +122,7 @@ __global__ void k_lw_merge(int D, int nblk, const float* __restrict__ covx, cons
     const float* blk = cov + (size_t)b * cstride;
     if (blk[0] == 0.f) continue;
     float fm, fc, nab;
-    lw_cgl(n, blk[0], fm, fc, nab);
+    cgl_factors(n, blk[0], fm, fc, nab);
     const float di = blk[2 + i] - mi, dj = blk[2 + j] - mj;
     m2 = m2 + blk[2 + D + (size_t)i * D + j] + di * dj * fc;
     mi = mi + di * fm;
@@ -489,8 +450,6 @@ __global__ void __launch_bounds__(kFinThreads) k_lw_final(int D, int k, float ga
   }
 }
 
-__global__ void k_lw_step_final(const float* __restrict__ st, float* __restrict__ out) { out[0] = expf(st[LW_LOG_AVG]); }
-
 // k_lrd_eig in its scatter mode on the symmetric W [D, D]: the top k eigenpairs by the largest eigenvalue into U [D, k]
 // (columns descending) and lam [k], warm-started from basis once hdr[LRD_WARM] is set
 int launch_lrd_eig_scatter(bjx_handle_t h, int D, int k, const float* W, float* hdr, float* U, float* lam, float* basis) {
@@ -533,7 +492,7 @@ extern "C" int bjx_lowrank_window_init(bjx_handle_t h, float* state, float initi
   const LwLayout L = lw_layout(C, D, k);
   BJX_CUDA(cudaMemsetAsync(state, 0, L.total * sizeof(float), h->stream));
   k_lw_init<<<1, 256, 0, h->stream>>>(D, k, state, initial_step_size, L);
-  k_lw_fill<<<(C + 255) / 256, 256, 0, h->stream>>>(C, state + LW_EPS, step_size_chain_out);
+  launch_fill_from(C, state + PS_EPS, step_size_chain_out, h->stream);
   BJX_CHECK_LAUNCH("k_lw_init");
   launch_lrd_install(D, k, state + L.sigma, state + L.U, state + L.lam, h->lr_block, h->stream);
   BJX_CHECK_LAUNCH("k_lrd_install");
@@ -566,7 +525,7 @@ extern "C" int bjx_lowrank_window_update(bjx_handle_t h, float* state, const flo
     BJX_CHECK_LAUNCH("k_cov_syrk");
   }
   k_lw_adapt<<<1, 32, 0, s>>>(L.nb, st + L.stx, 2 + 2 * (size_t)D, st, stage, window_end, target_acceptance, eps_history);
-  k_lw_fill<<<(C + 255) / 256, 256, 0, s>>>(C, st + LW_EPS, step_size_chain);
+  launch_fill_from(C, st + PS_EPS, step_size_chain, s);
   BJX_CHECK_LAUNCH("k_lw_adapt");
   if (!window_end) return 0;
   double* dbl = reinterpret_cast<double*>(st + L.dbl);
@@ -611,8 +570,8 @@ extern "C" int bjx_lowrank_window_final(bjx_handle_t h, const float* state, floa
   const int C = h->cfg.n_chains, D = h->cfg.dim;
   const LwLayout L = lw_layout(C, D, k);
   cudaStream_t s = h->stream;
-  k_lw_step_final<<<1, 1, 0, s>>>(state, step_size_out);
-  BJX_CHECK_LAUNCH("k_lw_step_final");
+  launch_da(3, 1, const_cast<float*>(state) + PS_DA, nullptr, 0.f, step_size_out, s);  // exp(log_step_avg)
+  BJX_CHECK_LAUNCH("k_da_final");
   BJX_CUDA(cudaMemcpyAsync(mu_star_out, state + L.mu, (size_t)D * sizeof(float), cudaMemcpyDeviceToDevice, s));
   BJX_CUDA(cudaMemcpyAsync(sigma_out, state + L.sigma, (size_t)D * sizeof(float), cudaMemcpyDeviceToDevice, s));
   BJX_CUDA(cudaMemcpyAsync(U_out, state + L.U, (size_t)D * k * sizeof(float), cudaMemcpyDeviceToDevice, s));

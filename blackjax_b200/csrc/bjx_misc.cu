@@ -72,40 +72,29 @@ void launch_diag_mass_sqrt(const float* imm, long long n, float* out, cudaStream
   if (n > 0) k_diag_mass_sqrt<<<grid1d(n), 256, 0, s>>>(imm, n, out);
 }
 
-// ---- dual averaging (optimizers/dual_averaging.py:87-129), one state per chain ---------------------------
-// state [C,5] = (log_step, log_step_avg, step, avg_error, mu)
+// ---- dual averaging (bjx_da.cuh), one state per chain: state [C,5] ---------------------------------------
 __global__ void k_da_init(int C, float* __restrict__ st, const float* __restrict__ eps0, float* __restrict__ eps_out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float x = eps0[c];
-  st[5 * c + 0] = logf(x);
-  st[5 * c + 1] = 0.f;
-  st[5 * c + 2] = 1.f;
-  st[5 * c + 3] = 0.f;
-  st[5 * c + 4] = logf(10.f * x);
-  if (eps_out) eps_out[c] = expf(st[5 * c + 0]);
+  da_init(st + 5 * c, eps0[c]);
+  if (eps_out) eps_out[c] = da_step_size(st + 5 * c);
 }
 __global__ void k_da_update(int C, float* __restrict__ st, const float* __restrict__ acc, float target,
                             float* __restrict__ eps_out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   da_update_step(st + 5 * c, acc[c], target);
-  if (eps_out) eps_out[c] = expf(st[5 * c + 0]);
+  if (eps_out) eps_out[c] = da_step_size(st + 5 * c);
 }
-__global__ void k_da_reset(int C, float* __restrict__ st, float* __restrict__ eps_out) {  // staged_adaptation.py:233-249
+__global__ void k_da_reset(int C, float* __restrict__ st, float* __restrict__ eps_out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float x = expf(st[5 * c + 1]);
-  st[5 * c + 0] = logf(x);
-  st[5 * c + 1] = 0.f;
-  st[5 * c + 2] = 1.f;
-  st[5 * c + 3] = 0.f;
-  st[5 * c + 4] = logf(10.f * x);
-  if (eps_out) eps_out[c] = expf(st[5 * c + 0]);
+  da_restart(st + 5 * c);
+  if (eps_out) eps_out[c] = da_step_size(st + 5 * c);
 }
 __global__ void k_da_final(int C, const float* __restrict__ st, float* __restrict__ eps_out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < C) eps_out[c] = expf(st[5 * c + 1]);
+  if (c < C) eps_out[c] = da_final(st + 5 * c);
 }
 void launch_da(int op, int C, float* st, const float* in, float target, float* eps_out, cudaStream_t s) {
   if (C <= 0) return;
