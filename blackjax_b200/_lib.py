@@ -38,6 +38,11 @@ class MclmcInfo(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("kinetic_change", "energy_change", "nonans")]
 
 
+class LapsBurnInConfig(C.Structure):
+    _fields_ = [("save_num", C.c_int32), ("alpha", C.c_float), ("C", C.c_float), ("r_end", C.c_float),
+                ("bias_type", C.c_int32), ("early_stop", C.c_int32), ("equi_full", C.c_int32)]
+
+
 class BjxError(RuntimeError):
     pass
 
@@ -98,6 +103,17 @@ _SIGNATURES = {
                                                           C.c_int32, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32,
                                                           C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                                           C.c_double, C.c_int64, _f32p]),
+    "bjx_laps_state_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "bjx_laps_init": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32]),
+    "bjx_laps_burn_in_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p,
+                                        _f32p, _f32p, C.POINTER(LapsBurnInConfig), _f32p]),
+    "bjx_laps_burn_in_run": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                       C.POINTER(LapsBurnInConfig), _f32p, C.c_int32, C.POINTER(C.c_int32)]),
+    "bjx_laps_switch": (C.c_int, [C.c_void_p, _f32p, C.c_int32]),
+    "bjx_laps_adjusted_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p,
+                                         _f32p, C.c_int32, C.c_int32, C.c_float, C.c_int32, _f32p]),
+    "bjx_laps_adjusted_run": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, _f32p, _f32p, _f32p, _f32p,
+                                        C.c_int32, C.c_int32, C.c_float, C.c_int32, _f32p]),
     "bjx_nuts_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
                                 C.c_int32, C.POINTER(Info), _f32p, _f32p]),
     "bjx_nuts_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, C.c_int32, _f32p,

@@ -11,7 +11,7 @@ namespace bjx {
 
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
 enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
-               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE };
+               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN };
 
 struct LaunchArgs {
   Params P;
@@ -23,7 +23,8 @@ struct LaunchArgs {
   AmclmcArgs amclmc;
   MclmcTuneArgs mclmc_tune;
   AmclmcTuneArgs amclmc_tune;
-  int grid_override;    // persistent launches: number of CTAs
+  LapsArgs laps;
+  int grid_override;   // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
   float *q_out, *logp_out, *g_out;
@@ -127,6 +128,13 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
     case K_AMCLMC_TUNE:  // diagonal metrics only, as K_MCLMC
       if constexpr (!DM) {
         k_amclmc_tune<R, TK, DM, GEN><<<grid, block, smem, st>>>(a.P, a.keys, a.q_out, a.logp_out, a.g_out, a.amclmc_tune);
+        return 0;
+      }
+      break;
+    case K_LAPS_BURN_IN:  // diagonal metrics only, as K_MCLMC; a fixed grid and the CTA's sums after the target's rows
+      if constexpr (!DM) {
+        k_laps_burn_in<R, TK, DM, GEN><<<laps_grid(a.P.C), block, smem + sizeof(float) * (3 * a.P.D + 4), st>>>(
+            a.P, a.q_out, a.p_io, a.logp_out, a.g_out, a.laps);
         return 0;
       }
       break;

@@ -428,6 +428,51 @@ int bjx_adjusted_mclmc_find_l_and_step_size(bjx_handle_t h, const uint32_t* rng_
                                             float target_num_integration_steps, double l_factor, int64_t max_history_bytes,
                                             float* num_integration_steps);
 
+/* ---- LAPS: the ensemble MCLMC warm-up (blackjax/adaptation/laps.py, laps_burn_in.py, eca.py) -------------------------
+ * One shared (step size, L, diagonal metric) for all chains of the handle, updated after every step from ensemble averages.
+ * state is a caller-owned float32 buffer of bjx_laps_state_floats(n_chains, dim, save_num, equi_full) floats (16-byte
+ * aligned) that carries the adaptation state and the scratch of both phases; save_num = rint(save_frac * num_steps1) >= 1.
+ * Every call on one state must pass the save_num it was sized with, and its burn-in steps the sizing's equi_full.
+ * phase_key is a HOST pointer to one raw key [2] (the phase's key1 / key2): chain c at step t uses
+ * fold_in(fold_in(key, 0), (chain_offset + c) T + t), equipartition_fullrank's probes fold_in(fold_in(key, 1), t).  The
+ * handle's metric must be the identity during the burn-in and the metric of the adjusted phase afterwards (the state's
+ * M^-1 = floats [16, 16 + dim), or ones), a shared diagonal metric [dim].  Supported configurations are those of
+ * bjx_mclmc_step with that metric kind (BJX_E_UNSUPPORTED otherwise). */
+typedef struct {
+  int32_t save_num;    /* rows of the history ring */
+  float alpha, C, r_end;
+  int32_t bias_type;   /* 0 r_max, 1 r_avg, 2 equi_full, 3 equi_diag */
+  int32_t early_stop;
+  int32_t equi_full;   /* compute equipartition_fullrank (required by bias_type 2) */
+} bjx_laps_burn_in_config;
+int64_t bjx_laps_state_floats(int32_t n_chains, int32_t dim, int32_t save_num, int32_t equi_full);
+/* laps_burn_in.initialize after sample_init: logp, grad = value_and_grad(q); u = grad / |grad| with dimension i's sign
+ * flipped when mean_c(-x_i g_i) < 1; the burn-in's initial adaptation state (L = inf, step size 0.01 sqrt(dim)). */
+int bjx_laps_init(bjx_handle_t h, const float* q, float* logp, float* grad, float* u, float* state, int32_t save_num);
+/* Burn-in step t of num_steps in place on (q, u, logp, grad, state): one fused MCLMC transition with nan_reject and the
+ * per-CTA sums, their merge, equipartition_fullrank if asked, and Adaptation.update with the stop rule.  info (optional,
+ * device, [num_steps, 9]) row t receives (L, step_size, EEVPD_wanted, EEVPD, equi_diag, equi_full, r_max, r_avg, entropy).
+ * After the stop every launch returns at once. */
+int bjx_laps_burn_in_step(bjx_handle_t h, const uint32_t* phase_key, int32_t t, int32_t num_steps, float* q, float* u,
+                          float* logp, float* grad, float* state, const bjx_laps_burn_in_config* cfg, float* info);
+/* All num_steps burn-in steps, reading the device's stop flag once per `chunk` steps (the result does not depend on chunk);
+ * *steps_run (host) receives the number of steps taken. */
+int bjx_laps_burn_in_run(bjx_handle_t h, const uint32_t* phase_key, int32_t num_steps, float* q, float* u, float* logp,
+                         float* grad, float* state, const bjx_laps_burn_in_config* cfg, float* info, int32_t chunk,
+                         int32_t* steps_run);
+/* laps.py:250-257: with diagonal_preconditioning, step size /= sqrt(mean(M^-1)); the bisection starts at [-inf, inf]. */
+int bjx_laps_switch(bjx_handle_t h, float* state, int32_t diagonal_preconditioning);
+/* Adjusted step t of num_samples in place on (q, logp, grad, state): one static adjusted MCLMC transition
+ * (steps_per_sample steps, L_proposal_factor 1.25, the state's step size, the handle's metric and integrator), the ensemble
+ * mean acceptance and bisection_monotonic_fn(target_acceptance).  info (optional, device, [num_samples, 4]) row t receives
+ * (L = step_size steps_per_sample, step_size, acc_prob, equi_diag); equi_diag is NaN and skipped without diagnostics. */
+int bjx_laps_adjusted_step(bjx_handle_t h, const uint32_t* phase_key, int32_t t, int32_t num_samples, float* q, float* logp,
+                           float* grad, float* state, int32_t save_num, int32_t steps_per_sample, float target_acceptance,
+                           int32_t diagnostics, float* info);
+int bjx_laps_adjusted_run(bjx_handle_t h, const uint32_t* phase_key, int32_t num_samples, float* q, float* logp,
+                          float* grad, float* state, int32_t save_num, int32_t steps_per_sample, float target_acceptance,
+                          int32_t diagnostics, float* info);
+
 /* ---- PRNG (jax.random restated; keys raw uint32 pairs) ----------------------------------------- */
 /* h may be NULL for the PRNG entry points: current device, and the stream this thread registered with
  * bjx_set_default_stream (a cudaStream_t; the legacy default stream until one is registered) */
