@@ -241,3 +241,6 @@ class _PerChainDiag(_Metric):
         self.imm = np.asarray(imm, F)
         self.dense = False
         self.mass_sqrt = (F(1.0) / np.sqrt(self.imm)).astype(F)
+
+    def chain(self, c):
+        return _Metric(self.imm[c])

@@ -37,6 +37,9 @@ class PerChainScale(Metric):
         self.dense = False
         self.mass_sqrt = (F(1.0) / np.sqrt(self.imm)).astype(F)   # metrics.py:699-704
 
+    def chain(self, c):
+        return Metric(self.imm[c])
+
 
 def init(position, target, keys):
     """ghmc.py:50-62.  keys uint32 [C, 2]."""

@@ -64,6 +64,11 @@ class Metric:
                 f" expected 1 or 2, got {imm.ndim}."
             )
 
+    def chain(self, c):
+        """The metric chain ``c`` runs with, for the single-chain code paths (the U-turn checkpoints of
+        oracle/nuts.py).  A shared metric is its own view; per-chain metrics return chain c's row."""
+        return self
+
     def velocity(self, p):
         """linear_map(M^-1, p) (util.py:57-61)."""
         if self.dense:

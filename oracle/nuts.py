@@ -45,7 +45,8 @@ def leaf_idx_to_ckpt_idxs(n):
 
 
 def is_iterative_turning(metric, ckpt_p, ckpt_sum, idx_min, idx_max, p_sum, p, margin=None):
-    """termination.py:86-104 for ONE chain (ckpt arrays [depth, D]).  ``margin``: 1-element array, lowered to the
+    """termination.py:86-104 for ONE chain (ckpt arrays [depth, D]; ``metric`` is that chain's, see
+    ``Metric.chain``).  ``margin``: 1-element array, lowered to the
     smallest relative distance of any evaluated U-turn product from its decision boundary (test aid)."""
     i = idx_max
     turning = False
@@ -138,7 +139,9 @@ def subtree(target, metric, keys, q, p, logp, g, direction, ckpt_p, ckpt_sum, ma
                 ckpt_p[c, idx_max] = np_[c]
                 ckpt_sum[c, idx_max] = new_sum[c]
             m1 = None if margins is None else margins[c:c + 1]
-            turning[c] = is_iterative_turning(metric, ckpt_p[c], ckpt_sum[c], idx_min, idx_max,
+            # chain c's own metric: a per-chain metric batched against one chain's vectors would broadcast the
+            # chain's momenta over every chain's inverse mass
+            turning[c] = is_iterative_turning(metric.chain(c), ckpt_p[c], ckpt_sum[c], idx_min, idx_max,
                                               new_sum[c], np_[c], m1)
         # commit for active chains only
         for k, v in zip(range(4), (nq, np_, nlogp, ng)):

@@ -6,7 +6,8 @@ rejects what it does not build: the general integrator and per-chain integration
 multinomial / generalized HMC, NUTS and the U-turn test on big rows, per-chain dense and low-rank metrics beyond their
 dims, a plug-in without the kernels of the row size.  This test creates handles over a grid of target x dim x metric x
 integrator that reaches every route and compares the return code of every entry point with tests/golden/routing_codes.json.
-The codes only say which calls are accepted; the numbers the calls produce are checked by the parity tests.
+The codes only say which calls are accepted; the numbers the calls produce are checked by the parity tests, those of the
+row kernels in every row size class (bjx_is_turning included) by tests/test_gpu_row_classes.py.
 """
 import ctypes as C
 import json
