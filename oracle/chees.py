@@ -17,7 +17,7 @@ Follows blackjax/adaptation/chees_adaptation.py:
 * run loop                 :737-1025 (jitter_gn, integration_steps_fn, one_step, final parameters; with the diagonal
                            metric the window starts at int(fraction * num_steps) and the eigenvalue is recomputed when
                            t % 32 == 0 in the window)
-* Halton sequence          blackjax/mcmc/dynamic_hmc.py:205-215
+* Halton sequence          blackjax/mcmc/dynamic_hmc.py:205-215 (adjusted_mclmc.halton_sequence)
 * dual averaging           blackjax/optimizers/dual_averaging.py:87-129 (gradient passed directly)
 * Adam                     optax.adam(learning_rate, b1, b2, eps=1e-8): scale_by_adam with bias correction, then -lr
                            (optax is a third-party dependency of the reference, absent from /root/reference; algorithm
@@ -32,6 +32,7 @@ import numpy as np
 
 from . import prng
 from .adaptation import DAState, cgl_update_batch, da_init, moment_block_init, welford_init, welford_update
+from .adjusted_mclmc import halton_sequence as halton
 from .hmc import F, hmc_kernel, init as hmc_init
 
 OPTIMAL_TARGET_ACCEPTANCE_RATE = 0.651
@@ -42,15 +43,6 @@ RECOMPUTE_INTERVAL = 32
 POWER_ITERATIONS = 5
 FINAL_POWER_ITERATIONS = 20
 LAMBDA_EPS = F(1e-6)
-
-
-def halton(i, max_bits=10):
-    """(i+1)-th element of the base-2 Halton sequence (dynamic_hmc.py:205-215); exact in float32."""
-    i = int(i)
-    s = F(0.0)
-    for k in range(int(max_bits)):
-        s = F(s + F(((i + 1) // (2 ** k)) % 2) * F(0.5 / 2 ** k))
-    return s
 
 
 def da_update_grad(s, gradient, t0=10, gamma=0.05, kappa=0.75):

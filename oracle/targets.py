@@ -12,6 +12,7 @@ integrators.py:189,204); without JAX the named models are differentiated by hand
 * ``NormLogpdf``                    tests/mcmc/test_trajectory.py:27 (jax.scipy.stats.norm.logpdf)
 * ``LinearRegression``              tests/mcmc/test_sampling.py:103-111 ``regression_logprob``
 * ``Rosenbrock``                    builder-defined neighbour-coupled model (blackjax_b200/user_targets/rosenbrock.cuh)
+* ``BoundedGaussian``               tests/mcmc/test_mclmc_nan_fix_969.py:45-47 (the bounded target of issue #969)
 
 Each target maps ``q: f32[C, D]`` to ``(logp: f32[C], grad: f32[C, D])``.
 """
@@ -249,3 +250,18 @@ class Rosenbrock:
             d[..., :-1] = F(-4.0) * a * xi * t - F(2.0) * o
             d[..., 1:] += F(2.0) * a * t
         return logp.astype(F), (-beta * d).astype(F)
+
+
+class BoundedGaussian:
+    """The bounded target of tests/mcmc/test_mclmc_nan_fix_969.py:45-47: -1/2 sum x^2 + sum log(B - |x|)."""
+
+    def __init__(self, dim, bound=5.0):
+        self.dim, self.bound = dim, F(bound)
+
+    def __call__(self, q):
+        q = np.asarray(q, F)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            r = (self.bound - np.abs(q)).astype(F)
+            logp = (F(-0.5) * np.sum(q * q, axis=-1, dtype=F) + np.sum(np.log(r), axis=-1, dtype=F)).astype(F)
+            g = (-q - np.where(q >= 0, F(1), F(-1)) / r).astype(F)
+        return logp, g

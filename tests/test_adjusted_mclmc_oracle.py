@@ -1,28 +1,21 @@
-"""CPU tests of the adjusted MCLMC / MAMS restatement (tests/helpers/adjusted_mclmc_oracle.py): its trajectory and energy
+"""CPU tests of the adjusted MCLMC / MAMS restatement (oracle/adjusted_mclmc.py): its trajectory and energy
 difference against explicit compositions of the MCLMC oracle's integrator step, the key tree at n = 0, the step-count rules
 (rescale, the Halton lengths), a long run on a small Gaussian (and the bias of unadjusted MCLMC at the same step size that
-the adjustment removes), the Python surface of blackjax_b200.adjusted_mclmc / adjusted_mclmc_dynamic without a GPU, and
-the transition kernel's compile (sm_90a, no local-memory spills)."""
+the adjustment removes), and the Python surface of blackjax_b200.adjusted_mclmc / adjusted_mclmc_dynamic without a
+GPU."""
 import math
-import os
-import re
-import shutil
-import subprocess
-import sys
 import warnings
 
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import adjusted_mclmc_oracle as oa  # noqa: E402
-import mclmc_oracle as om  # noqa: E402
-from oracle import prng as oprng  # noqa: E402
-from oracle import targets as otargets  # noqa: E402
+from oracle import adjusted_mclmc as oa
+from oracle import mclmc as om
+from oracle import prng as oprng
+from oracle import targets as otargets
 
 F = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MCLACHLAN = (0.1931833275037836, 0.5, 1.0 - 2 * 0.1931833275037836, 0.5, 0.1931833275037836)
 VELOCITY_VERLET = (0.5, 1.0, 0.5)
 
@@ -232,32 +225,3 @@ def test_python_surface_without_gpu():
     assert fixed(None, 3.2) == 4 and fixed(None, 0.3) == 1
     assert amd.make_random_trajectory_length_fn(True).device_rule == (2, 1)
     assert amd.make_random_trajectory_length_fn(True, min_steps=0).device_rule == (2, 0)
-
-
-_INSTANCES = [(r, "TK_DIAG") for r in ("Row<1, false>", "Row<4, false>", "Row<4, true>", "Row<8, true>", "Row<16, true>",
-                                       "Row<32, true>")] + [("Row<32, true>", "TK_FUNNEL"), ("Row<4, true>", "TK_DENSE"),
-                                                            ("Row<1, false>", "TK_BANANA")]
-
-
-def _spill_source():
-    lines = ['#include "bjx_kernels.cuh"', "namespace bjx {"]
-    for row, tk in _INSTANCES:
-        for gen in ("false", "true"):
-            lines.append(f"template __global__ void k_amclmc_transition<{row}, {tk}, false, {gen}>(Params, const uint32_t*, "
-                         "const float*, const float*, const float*, float*, float*, float*, AmclmcArgs, InfoPtrs);")
-    return "\n".join(lines + ["}"]) + "\n"
-
-
-@pytest.mark.skipif(shutil.which("nvcc") is None and not os.path.exists("/usr/local/cuda/bin/nvcc"), reason="needs nvcc")
-def test_adjusted_mclmc_kernel_compiles_without_spills(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    src = tmp_path / "amclmc_inst.cu"
-    src.write_text(_spill_source())
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                          "-I", os.path.join(ROOT, "blackjax_b200", "csrc"), "-c", str(src), "-o", str(tmp_path / "a.o")],
-                         capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    blocks = [b for b in re.split(r"Compiling entry function", out.stderr) if "k_amclmc_transition" in b.split("\n")[0]]
-    assert len(blocks) == 2 * len(_INSTANCES), [b.split("\n")[0] for b in blocks]
-    for b in blocks:
-        assert "0 bytes spill stores, 0 bytes spill loads" in b and "0 bytes stack frame" in b, b

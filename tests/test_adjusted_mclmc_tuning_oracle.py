@@ -1,27 +1,23 @@
-"""CPU tests of the adjusted MCLMC tuner's restatement (tests/helpers/adjusted_mclmc_tuning_oracle.py): stage lengths,
+"""CPU tests of the adjusted MCLMC tuner's restatement (oracle/adjusted_mclmc_tuning.py): stage lengths,
 the masked dual averaging with its clamp and log round trip, the L / step-size update order, the key tree against an explicit
 oprng composition, handle_nans' revert, the exit invariant, the reference's L / step = 2.0 and 1.5 assertions at D = 5, and
 the Python surface of blackjax_b200.adjusted_mclmc_find_L_and_step_size without a GPU, and a spill-free sm_90a compile of
 every instance of the fused tuning step beside the transition it shares its body with."""
 import inspect
 import os
-import re
-import shutil
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import adjusted_mclmc_oracle as ao  # noqa: E402
-import adjusted_mclmc_tuning_oracle as at  # noqa: E402
-from oracle import prng as oprng  # noqa: E402
-from oracle import targets as otargets  # noqa: E402
-from oracle.adaptation import DAState, da_init, da_update  # noqa: E402
+from oracle import adjusted_mclmc as ao
+from oracle import adjusted_mclmc_tuning as at
+from oracle import prng as oprng
+from oracle import targets as otargets
+from oracle.adaptation import DAState, da_init, da_update
+from test_kernel_spills import (AMCLMC_TRANSITION, INSTANCES, NVCC, WITH_CSRC, assert_entries_clean, instantiate,
+                                ptxas_log)
 
 F = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MCLACHLAN = (0.1931833275037836, 0.5, 1.0 - 2 * 0.1931833275037836, 0.5, 0.1931833275037836)
 UNIFORM0 = ("uniform", 0)  # the reference tests' ceil(uniform(key) * rescale(avg)), unclipped
 
@@ -195,30 +191,9 @@ def test_rescale_matches_the_sampler_restatement():
             ao.steps_uniform(oprng.split(oprng.key(1), 1), mu, 0)[0]
 
 
-_INSTANCES = [(r, "TK_DIAG") for r in ("Row<1, false>", "Row<4, false>", "Row<4, true>", "Row<8, true>", "Row<16, true>",
-                                       "Row<32, true>")] + [("Row<32, true>", "TK_FUNNEL"), ("Row<4, true>", "TK_DENSE"),
-                                                            ("Row<1, false>", "TK_BANANA")]
-
-
-@pytest.mark.skipif(shutil.which("nvcc") is None and not os.path.exists("/usr/local/cuda/bin/nvcc"), reason="needs nvcc")
+@pytest.mark.skipif(not os.path.exists(NVCC), reason="needs nvcc")
 def test_tuning_step_compiles_without_spills(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    lines = ['#include "bjx_kernels.cuh"', "namespace bjx {"]
-    for row, tk in _INSTANCES:
-        for gen in ("false", "true"):
-            lines.append(f"template __global__ void k_amclmc_tune<{row}, {tk}, false, {gen}>(Params, const uint32_t*, "
-                         "float*, float*, float*, AmclmcTuneArgs);")
-            lines.append(f"template __global__ void k_amclmc_transition<{row}, {tk}, false, {gen}>(Params, "
-                         "const uint32_t*, const float*, const float*, const float*, float*, float*, float*, AmclmcArgs, "
-                         "InfoPtrs);")
-    src = tmp_path / "amclmc_tune_inst.cu"
-    src.write_text("\n".join(lines + ["}"]) + "\n")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                          "-I", os.path.join(ROOT, "blackjax_b200", "csrc"), "-c", str(src), "-o", str(tmp_path / "a.o")],
-                         capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    blocks = [b for b in re.split(r"Compiling entry function", out.stderr)
-              if "k_amclmc_tune" in b.split("\n")[0] or "k_amclmc_transition" in b.split("\n")[0]]
-    assert len(blocks) == 4 * len(_INSTANCES), [b.split("\n")[0] for b in blocks]
-    for b in blocks:
-        assert "0 bytes spill stores, 0 bytes spill loads" in b and "0 bytes stack frame" in b, b
+    src = instantiate(("k_amclmc_tune", "Params, const uint32_t*, float*, float*, float*, AmclmcTuneArgs"),
+                      AMCLMC_TRANSITION)
+    log = ptxas_log(tmp_path, src, WITH_CSRC)
+    assert_entries_clean(log, ("k_amclmc_tune", "k_amclmc_transition"), 4 * len(INSTANCES))

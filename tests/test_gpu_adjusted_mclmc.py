@@ -1,5 +1,5 @@
 """Adjusted MCLMC / MAMS on the GPU (k_amclmc_transition through bjx_adjusted_mclmc_step / bjx_adjusted_mclmc_sample)
-against the float32 restatement in tests/helpers/adjusted_mclmc_oracle.py on the same state and keys.
+against the float32 restatement in oracle/adjusted_mclmc.py on the same state and keys.
 
 * one transition, teacher-forced: the proposal (q, unit momentum), the drawn momentum, energy, and the new q, logp, grad
   within 1e-5 relative (close() of test_gpu_parity), p_accept within 1e-5 of the log-density scale, and accept decisions
@@ -15,8 +15,6 @@ against the float32 restatement in tests/helpers/adjusted_mclmc_oracle.py on the
 * the reference's regression posterior (tests/mcmc/test_sampling.py:432-480), static and dynamic.
 """
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
@@ -26,12 +24,10 @@ import blackjax_b200 as bj
 from blackjax_b200 import _lib, plugin, targets as T
 from blackjax_b200.mcmc import adjusted_mclmc_dynamic as amd
 from blackjax_b200.mcmc import integrators
+from oracle import adjusted_mclmc as oa
 from oracle import prng as oprng
 from oracle import targets as otargets
 from test_gpu_parity import close, npy, tf, tk
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import adjusted_mclmc_oracle as oa  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 F = np.float32

@@ -1,5 +1,5 @@
 """Adjusted MCLMC's tuner on the GPU (k_amclmc_tune and bjx_adjusted_mclmc_find_l_and_step_size) against the float32
-restatement in tests/helpers/adjusted_mclmc_tuning_oracle.py.
+restatement in oracle/adjusted_mclmc_tuning.py.
 
 * one tuning step, teacher-forced: step counts and success flags exact; the state within close() of the oracle; the DA
   fields, eps, L, the streaming total and moments within 1e-5 of the oracle's update fed with the device's own transition
@@ -11,8 +11,6 @@ restatement in tests/helpers/adjusted_mclmc_tuning_oracle.py.
 * rejections.
 """
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
@@ -23,14 +21,12 @@ from blackjax_b200 import _engine, _lib, plugin, targets as T
 from blackjax_b200.adaptation import adjusted_mclmc_adaptation as ama
 from blackjax_b200.mcmc import adjusted_mclmc_dynamic as amd
 from blackjax_b200.mcmc import integrators
+from oracle import adjusted_mclmc as ao
+from oracle import adjusted_mclmc_tuning as at
 from oracle import prng as oprng
 from oracle import targets as otargets
 from oracle.adaptation import da_init
 from test_gpu_parity import close, npy, tf, tk
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import adjusted_mclmc_oracle as ao  # noqa: E402
-import adjusted_mclmc_tuning_oracle as at  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 F = np.float32

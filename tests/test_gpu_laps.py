@@ -1,10 +1,8 @@
-"""LAPS on the GPU (bjx_laps_*, k_laps_burn_in) against the NumPy restatement in tests/helpers/laps_oracle.py:
+"""LAPS on the GPU (bjx_laps_*, k_laps_burn_in) against the NumPy restatement in oracle/laps.py:
 initialisation, teacher-forced burn-in steps and their ensemble update, equipartition_fullrank, bit identity (chunk size,
 diagnostics, repeated runs), the adjusted phase against bjx_adjusted_mclmc_step and the bisection, the phase-boundary
 choices, a recovery test on a badly scaled Gaussian and the rejections."""
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
@@ -15,12 +13,10 @@ from blackjax_b200 import _engine, _lib, plugin, targets as T
 from blackjax_b200.adaptation import laps as L
 from blackjax_b200.adaptation import laps_burn_in as lb
 from blackjax_b200.mcmc import integrators
+from oracle import laps as ol
 from oracle import prng as oprng
 from oracle import targets as otargets
 from test_gpu_parity import close, npy, tf, tk
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import laps_oracle as ol  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 F = np.float32

@@ -1,5 +1,5 @@
 """MCLMC on the GPU (k_mclmc_transition through bjx_mclmc_init / bjx_mclmc_step / bjx_mclmc_sample) against the float32
-restatement in tests/helpers/mclmc_oracle.py on the same state and keys.
+restatement in oracle/mclmc.py on the same state and keys.
 
 * init: the momentum is the oracle's unit vector within 1e-6;
 * one transition, teacher-forced: q, p, logp, grad and the energy change within 1e-5 relative (close(): abs floor 5 % of the
@@ -16,8 +16,6 @@ restatement in tests/helpers/mclmc_oracle.py on the same state and keys.
 * a long run on a scaled Gaussian recovers its mean and variance.
 """
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
@@ -26,12 +24,10 @@ import torch
 import blackjax_b200 as bj
 from blackjax_b200 import _lib, plugin, targets as T
 from blackjax_b200.mcmc import integrators
+from oracle import mclmc as om
 from oracle import prng as oprng
 from oracle import targets as otargets
 from test_gpu_parity import close, npy, tf, tk
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import mclmc_oracle as om  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -237,7 +233,7 @@ def test_nan_cases_revert(table, step_size, seeds):
     ks = np.stack([oprng.split(oprng.key(s), 2) for s in seeds])
     init_keys, step_keys = ks[:, 0], ks[:, 1]
     C = len(ks)
-    tgt, otgt = _bounded(), om.BoundedGaussian(2)
+    tgt, otgt = _bounded(), otargets.BoundedGaussian(2)
     st = bj.mclmc.init(tf(np.zeros((C, 2))), tgt, tk(init_keys))
     new, info = bj.mclmc.build_kernel(integrator=TABLES[table])(tk(step_keys), st, tgt, 1.0, 1.0, step_size)
     ostate = om.mclmc_init(np.zeros((C, 2), F), otgt, init_keys)

@@ -1,5 +1,5 @@
 """MCLMC's tuner on the GPU (k_mclmc_tune, k_ess_chain and bjx_mclmc_find_l_and_step_size) against the float32 restatement
-in tests/helpers/mclmc_tuning_oracle.py.
+in oracle/mclmc_tuning.py.
 
 * one tuning step, teacher-forced: state within close() of the oracle, success identical; the new step size, time,
   x_average, step_size_max and the streaming weight within 1e-5 relative, and the moment rows within close(), of the
@@ -13,8 +13,6 @@ in tests/helpers/mclmc_tuning_oracle.py.
 * the reference's statistical tests, every chain tuning on its own.
 """
 import math
-import os
-import sys
 
 import numpy as np
 import pytest
@@ -24,14 +22,12 @@ import blackjax_b200 as bj
 from blackjax_b200 import _engine, _lib, plugin, targets as T
 from blackjax_b200.adaptation import mclmc_adaptation as ma
 from blackjax_b200.mcmc import integrators
+from oracle import mclmc as om
+from oracle import mclmc_tuning as ot
 from oracle import prng as oprng
 from oracle import targets as otargets
 from oracle.diagnostics import effective_sample_size as oracle_ess
 from test_gpu_parity import close, npy, tf, tk
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import mclmc_oracle as om  # noqa: E402
-import mclmc_tuning_oracle as ot  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -148,7 +144,7 @@ def test_tune_step_failures_on_the_bounded_target(table):
     """#969: step size 100 / 8 on the bounded target; failed chains keep their whole state, momentum included, and take
     step_size_max = 0.8 eps."""
     C = 64
-    tgt, otgt = _bounded(), om.BoundedGaussian(2)
+    tgt, otgt = _bounded(), otargets.BoundedGaussian(2)
     init_keys = oprng.split(oprng.key(3), C)
     ostate = om.mclmc_init(np.zeros((C, 2), F), otgt, init_keys)
     eps = np.full(C, 100.0 if table == "mclachlan" else 8.0, F)
@@ -335,8 +331,9 @@ def test_convergence_from_large_step_size_on_the_bounded_target(table):
     inside = (eps >= 0.1) & (eps <= 10.0)
     assert inside.mean() >= 0.98, eps[~inside]
     ck = oprng.fold_in(oprng.key(100), np.arange(C))
-    ost = om.mclmc_init(np.zeros((C, 2), F), om.BoundedGaussian(2), ck)
-    _, (_, oeps, _), _, _ = ot.find_L_and_step_size(ck, 60, ost, om.BoundedGaussian(2), TABLES[table], frac_tune1=1.0,
-                                                    frac_tune2=0.0, frac_tune3=0.0, diagonal_preconditioning=False,
+    ost = om.mclmc_init(np.zeros((C, 2), F), otargets.BoundedGaussian(2), ck)
+    _, (_, oeps, _), _, _ = ot.find_L_and_step_size(ck, 60, ost, otargets.BoundedGaussian(2), TABLES[table],
+                                                    frac_tune1=1.0, frac_tune2=0.0, frac_tune3=0.0,
+                                                    diagonal_preconditioning=False,
                                                     params=(np.sqrt(F(2)), F(100), np.ones(2, F)))
     assert np.array_equal(inside, (oeps >= 0.1) & (oeps <= 10.0))

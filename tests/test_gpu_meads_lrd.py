@@ -1,9 +1,7 @@
 """GPU tests of MEADS-LRD (meads_adaptation(..., low_rank_rank=k)): the on-device eigensolver of bjx_meads_lrd_update /
 bjx_meads_lrd_metric against float64 numpy.linalg.eigh, one warm-up step's statistics teacher-forced against
-tests/helpers/meads_lrd_oracle.py, and the reference's low-rank MEADS tests (tests/adaptation/test_meads.py
+oracle/meads_lrd.py, and the reference's low-rank MEADS tests (tests/adaptation/test_meads.py
 TestMEADSLowRank, TestMEADSLowRankHighDimFixes, TestMEADSLRDX64Sanity) replayed on the device."""
-import os
-import sys
 import warnings
 
 import numpy as np
@@ -14,9 +12,7 @@ import blackjax_b200 as bj
 from blackjax_b200 import _engine, targets as T
 from blackjax_b200.adaptation import meads_adaptation as mm
 from blackjax_b200.mcmc.metrics import LowRankMetric
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import meads_lrd_oracle as olrd  # noqa: E402
+from oracle import meads_lrd as olrd
 
 pytestmark = pytest.mark.gpu
 F = np.float32

@@ -238,7 +238,7 @@ def test_nuts_runs_without_host_round_trips_and_reports_depth_on_request():
 
 
 # ---------------------------------------------------------------------------------------------------------
-# ADVICE: PRNG helpers on side streams; metric cache keyed on content version
+# ADVICE: PRNG calls on side streams; metric cache keyed on content version
 # ---------------------------------------------------------------------------------------------------------
 def test_prng_and_warmup_inside_a_side_stream():
     s = torch.cuda.Stream(device=DEV)

@@ -126,7 +126,7 @@ check_homes([(D, depth, False) for D, depth in EXACT_CASES], "EXACT_CASES")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# helpers
+# setup shared by the tests below
 # ---------------------------------------------------------------------------------------------------------------------
 def make_metric(kind, D, C, rs):
     """(device metric, oracle metric) of one kind."""

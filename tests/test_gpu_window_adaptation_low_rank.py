@@ -1,10 +1,7 @@
 """GPU tests of window_adaptation_low_rank: the device fold and window-end estimator teacher-forced against the float64
-oracle (tests/helpers/low_rank_window_oracle.py), the whole update loop teacher-forced under Stan's and the growing
+oracle (oracle/low_rank_window.py), the whole update loop teacher-forced under Stan's and the growing
 schedule, the reference's statistical tests (tests/adaptation/test_low_rank_adaptation.py) pooled over chains, bit
 identity and the rejections."""
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -14,9 +11,7 @@ from blackjax_b200 import _engine, targets as T
 from blackjax_b200._lib import BjxError
 from blackjax_b200.adaptation import low_rank_adaptation as lra
 from blackjax_b200.mcmc.metrics import LowRankMetric
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import low_rank_window_oracle as o  # noqa: E402
+from oracle import low_rank_window as o
 
 pytestmark = pytest.mark.gpu
 F = np.float32

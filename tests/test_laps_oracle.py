@@ -1,14 +1,10 @@
-"""CPU tests of the LAPS restatement (tests/helpers/laps_oracle.py): the reference's #969 known answer, the history and
+"""CPU tests of the LAPS restatement (oracle/laps.py): the reference's #969 known answer, the history and
 its contraction, the bisection, the early-stop index, the key layout and rademacher."""
-import os
-import sys
-
 import numpy as np
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import laps_oracle as ol  # noqa: E402
-import mclmc_oracle as om  # noqa: E402
-from oracle import prng as oprng  # noqa: E402
+from oracle import laps as ol
+from oracle import prng as oprng
+from oracle import targets as otargets
 
 F = np.float32
 
@@ -17,7 +13,7 @@ def test_nan_fix_969_halves_the_step_size():
     """tests/mcmc/test_mclmc_nan_fix_969.py:253-295: at eps = 100 on the bounded target some chains report NaN, keep their
     state and the update halves the step size."""
     N, D = 16, 2
-    tgt = om.BoundedGaussian(D)
+    tgt = otargets.BoundedGaussian(D)
     q = (0.5 * np.random.default_rng(0).standard_normal((N, D))).astype(F)
     state, _ = ol.initialize(q, tgt)
     ad = ol.BurnIn(D, 2)

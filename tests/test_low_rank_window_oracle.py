@@ -1,21 +1,12 @@
-"""CPU tests of the low-rank window adaptation's oracle (tests/helpers/low_rank_window_oracle.py) -- the reference's own
+"""CPU tests of the low-rank window adaptation's oracle (oracle/low_rank_window.py) -- the reference's own
 known answers (tests/adaptation/test_low_rank_adaptation.py) -- of the accumulator form the device computes, of the
-package's schedule and retained-step rule, of the argument checks, and of the sm_90a compile of the new kernels."""
-import os
-import shutil
-import subprocess
-import sys
-
+package's schedule and retained-step rule, and of the argument checks."""
 import numpy as np
 import pytest
 
 import blackjax_b200 as bj
 from blackjax_b200.adaptation import low_rank_adaptation as lra
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import low_rank_window_oracle as o  # noqa: E402
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from oracle import low_rank_window as o
 
 
 def spd(rs, n):
@@ -183,18 +174,3 @@ def test_rejections_without_gpu():
         bj.window_adaptation_low_rank(bj.hmc, tgt)   # no num_integration_steps
     with pytest.raises(ValueError):
         lra.schedule_bytes([(0, True)], 1)
-
-
-def test_low_rank_window_kernels_compile_without_spills(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    src = os.path.join(ROOT, "blackjax_b200", "csrc")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                          "-I", os.path.join(ROOT, "include"), "-c", os.path.join(src, "bjx_lowrank_window.cu"),
-                          "-o", str(tmp_path / "lw.o")], capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr
-    log = out.stderr
-    assert "k_lw_final" in log and "k_lw_merge" in log
-    spills = [ln for ln in log.splitlines() if "spill" in ln and not ln.strip().startswith("0 bytes spill")]
-    assert not [ln for ln in spills if " 0 bytes spill stores, 0 bytes spill loads" not in ln], spills

@@ -1,24 +1,17 @@
-"""CPU tests of the MCLMC restatement (tests/helpers/mclmc_oracle.py) against the reference's own known-answer tests
-(tests/mcmc/test_integrators.py:225-349, tests/mcmc/test_mclmc_nan_fix_969.py:82-119), the Python-side argument handling
-of blackjax_b200.mclmc, and the transition kernel's compile (sm_90a, no local-memory spills)."""
+"""CPU tests of the MCLMC restatement (oracle/mclmc.py) against the reference's own known-answer tests
+(tests/mcmc/test_integrators.py:225-349, tests/mcmc/test_mclmc_nan_fix_969.py:82-119), and the Python-side argument
+handling of blackjax_b200.mclmc."""
 import math
-import os
-import re
-import shutil
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "helpers"))
-import mclmc_oracle as om  # noqa: E402
-from oracle import prng as oprng  # noqa: E402
-from oracle import targets as otargets  # noqa: E402
+from oracle import mclmc as om
+from oracle import prng as oprng
+from oracle import targets as otargets
 
 F = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TABLES = {"velocity_verlet": (0.5, 1.0, 0.5),
           "mclachlan": (0.1931833275037836, 0.5, 1.0 - 2 * 0.1931833275037836, 0.5, 0.1931833275037836)}
 _b1y, _a1y = 0.11888010966548, 0.29619504261126
@@ -85,7 +78,7 @@ def test_isokinetic_integrator_conserves_energy(table):
 
 
 def _bounded_kernel(seed, table, step_size):
-    target = om.BoundedGaussian(2)
+    target = otargets.BoundedGaussian(2)
     init_key, step_key = oprng.split(oprng.key(seed), 2)
     state = om.mclmc_init(np.zeros((1, 2), F), target, init_key[None])
     return om.mclmc_kernel(step_key[None], state, target, np.ones(2, F), F(1.0), F(step_size), TABLES[table])
@@ -135,33 +128,3 @@ def test_python_surface_without_gpu():
     with pytest.raises(ValueError, match="more than 1 dimension"):
         bj.mclmc.init(torch.zeros(4, 1), bj.targets.StdNormal(1), torch.zeros(2, dtype=torch.uint32))
     assert set(bj.mcmc.mclmc.MCLMCInfo._fields) == {"logdensity", "kinetic_change", "energy_change", "nonans"}
-
-
-# every row size class with the diagonal Gaussian, plus the other built-in targets at the size classes they run on
-_INSTANCES = [(r, "TK_DIAG") for r in ("Row<1, false>", "Row<4, false>", "Row<4, true>", "Row<8, true>", "Row<16, true>",
-                                       "Row<32, true>")] + [("Row<32, true>", "TK_FUNNEL"), ("Row<4, true>", "TK_DENSE"),
-                                                            ("Row<1, false>", "TK_BANANA")]
-
-
-def _spill_source():
-    lines = ['#include "bjx_kernels.cuh"', "namespace bjx {"]
-    for row, tk in _INSTANCES:
-        for gen in ("false", "true"):
-            lines.append(f"template __global__ void k_mclmc_transition<{row}, {tk}, false, {gen}>(Params, const uint32_t*, "
-                         "float*, float*, float*, float*, MclmcArgs);")
-    return "\n".join(lines + ["}"]) + "\n"
-
-
-@pytest.mark.skipif(shutil.which("nvcc") is None and not os.path.exists("/usr/local/cuda/bin/nvcc"), reason="needs nvcc")
-def test_mclmc_kernel_compiles_without_spills(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    src = tmp_path / "mclmc_inst.cu"
-    src.write_text(_spill_source())
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v",
-                          "-I", os.path.join(ROOT, "blackjax_b200", "csrc"), "-c", str(src), "-o", str(tmp_path / "m.o")],
-                         capture_output=True, text=True)
-    assert out.returncode == 0, out.stderr[-2000:]
-    blocks = [b for b in re.split(r"Compiling entry function", out.stderr) if "k_mclmc_transition" in b.split("\n")[0]]
-    assert len(blocks) == 2 * len(_INSTANCES), [b.split("\n")[0] for b in blocks]
-    for b in blocks:
-        assert "0 bytes spill stores, 0 bytes spill loads" in b and "0 bytes stack frame" in b, b
