@@ -25,7 +25,9 @@ from .mcmc import mclmc as _mclmc
 from .mcmc import adjusted_mclmc as _adjusted_mclmc
 from .mcmc import adjusted_mclmc_dynamic as _adjusted_mclmc_dynamic
 from .util import run_inference_algorithm, sample_hmc_native, sample_mclmc_native, sample_nuts_native  # noqa: F401
-from .util import sample_adjusted_mclmc_native  # noqa: F401
+from .util import sample_adjusted_mclmc_native, sample_gist_native  # noqa: F401
+from .mcmc.composed import step_size as _gist_step_size
+from .mcmc.composed import trajectory_length as _gist_trajectory_length
 
 hmc = GenerateSamplingAPI(_hmc.as_top_level_api, _hmc.init, _hmc.build_kernel)     # blackjax/__init__.py:111
 nuts = GenerateSamplingAPI(_nuts.as_top_level_api, _nuts.init, _nuts.build_kernel)  # blackjax/__init__.py:112
@@ -49,5 +51,9 @@ adjusted_mclmc = GenerateSamplingAPI(_adjusted_mclmc.as_top_level_api, _adjusted
                                      _adjusted_mclmc.build_kernel)
 adjusted_mclmc_dynamic = GenerateSamplingAPI(_adjusted_mclmc_dynamic.as_top_level_api, _adjusted_mclmc_dynamic.init,
                                              _adjusted_mclmc_dynamic.build_kernel)
+gist_trajectory_length = GenerateSamplingAPI(_gist_trajectory_length.as_top_level_api,  # blackjax/__init__.py:143
+                                             _gist_trajectory_length.init, _gist_trajectory_length.build_kernel)
+gist_step_size = GenerateSamplingAPI(_gist_step_size.as_top_level_api, _gist_step_size.init,  # blackjax/__init__.py:142
+                                     _gist_step_size.build_kernel)
 
 __version__ = "0.1.0"

@@ -316,6 +316,20 @@ class Engine:
         self._amclmc_keepalive = (steps_dev, eps_dev, avg_dev)  # the launch is asynchronous: keep the arrays
         return qo, lo, go
 
+    def gist_step(self, keys, q, logp, g, params, step_size, out=None, info_fields=None, chain_offset=0):
+        """One GIST transition (libbjx ``bjx_gist_step``); ``params`` is a ``_lib.GistParams``."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        g = _f32(g, (self.C, self.D), "logdensity_grad")
+        logp = _f32(logp, (self.C,), "logdensity")
+        qo, lo, go = out if out is not None else (torch.empty_like(q), torch.empty_like(logp), torch.empty_like(g))
+        eps, eps_dev = self._eps(step_size)
+        info = self._info(info_fields or {}, _lib.GistInfo)
+        check(lib().bjx_gist_step(self.h, C.byref(params), ptr(keys), ptr(q), ptr(logp), ptr(g), ptr(qo), ptr(lo),
+                                  ptr(go), eps, ptr(eps_dev), C.byref(info)), self.h)
+        return qo, lo, go
+
     def adjusted_mclmc_num_steps(self, device_rule, avg, random_generator_arg):
         """The step counts int32 [C] of a dynamic rule ``device_rule = (rule, min_steps)`` at a per-chain ``avg`` [C]
         (libbjx ``bjx_adjusted_mclmc_num_steps``); random_generator_arg [C, 2] is read, not advanced.  The fixed rule

@@ -10,6 +10,8 @@ TARGET_DIAG_GAUSSIAN, TARGET_FUNNEL, TARGET_DENSE_GAUSSIAN, TARGET_BANANA, TARGE
 METRIC_DIAG, METRIC_DENSE, METRIC_DIAG_PER_CHAIN, METRIC_LOW_RANK, METRIC_DENSE_PER_CHAIN = 0, 1, 2, 3, 4
 CHEES_WHITEN, CHEES_LENGTH_FLOOR = 1, 2
 AMCLMC_STEPS_FIXED, AMCLMC_STEPS_RANDINT, AMCLMC_STEPS_UNIFORM = 0, 1, 2
+GIST_TRAJECTORY_LENGTH, GIST_STEP_SIZE = 0, 1
+GIST_SYMMETRIC, GIST_ASYMMETRIC = 0, 1
 
 _f32p = C.c_void_p  # device pointers travel as integers
 
@@ -36,6 +38,17 @@ class Info(C.Structure):
 
 class MclmcInfo(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("kinetic_change", "energy_change", "nonans")]
+
+
+class GistParams(C.Structure):
+    _fields_ = [("instance", C.c_int32), ("path_fraction", C.c_float), ("max_num_steps", C.c_int32),
+                ("num_integration_steps", C.c_int32), ("max_search_steps", C.c_int32), ("criterion", C.c_int32)]
+
+
+class GistInfo(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in (
+        "acceptance_rate", "is_accepted", "is_divergent", "energy", "momentum", "num_integration_steps", "forward",
+        "reverse", "rejected", "a", "b", "step_size")]
 
 
 class LapsBurnInConfig(C.Structure):
@@ -103,6 +116,10 @@ _SIGNATURES = {
                                                           C.c_int32, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, C.c_int32,
                                                           C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                                           C.c_double, C.c_int64, _f32p]),
+    "bjx_gist_step": (C.c_int, [C.c_void_p, C.POINTER(GistParams), _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p,
+                                C.c_float, _f32p, C.POINTER(GistInfo)]),
+    "bjx_gist_sample": (C.c_int, [C.c_void_p, C.POINTER(GistParams), _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
+                                  C.c_int32, _f32p, C.c_int32, _f32p, C.c_void_p]),
     "bjx_laps_state_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "bjx_laps_init": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32]),
     "bjx_laps_burn_in_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p,

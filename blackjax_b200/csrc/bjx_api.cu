@@ -177,6 +177,7 @@ extern "C" int bjx_destroy(bjx_handle_t h) {
   if (h->lr_block) cudaFree(h->lr_block);
   if (h->gemm_ws) cudaFree(h->gemm_ws);
   if (h->sample_keys) cudaFree(h->sample_keys);
+  if (h->gist_ws) cudaFree(h->gist_ws);
   if (h->h_flag) cudaFreeHost(h->h_flag);
   delete h;
   return 0;

@@ -58,6 +58,8 @@ struct bjx_handle_s {
   uint32_t chain_offset = 0;
   uint32_t* sample_keys = nullptr;     // [num_steps, 2] step keys of the run loops (bjx_hmc_sample, ...)
   size_t sample_keys_cap = 0;
+  float* gist_ws = nullptr;            // GIST scratch (bjx_gist.cu): 4 rows [C,D] and the chain queue
+  size_t gist_ws_cap = 0;
   std::string err;
 };
 

@@ -11,7 +11,7 @@ namespace bjx {
 
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
 enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
-               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN };
+               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN, K_GIST, K_GIST_CHAINS };
 
 struct LaunchArgs {
   Params P;
@@ -24,6 +24,7 @@ struct LaunchArgs {
   MclmcTuneArgs mclmc_tune;
   AmclmcTuneArgs amclmc_tune;
   LapsArgs laps;
+  GistArgs gist;
   int grid_override;   // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
@@ -76,6 +77,13 @@ struct Launcher {
 #ifndef BJX_BUILD_GEN
 #define BJX_BUILD_GEN 2   // 0: velocity Verlet only; 1: general coefficient tables only; 2: both
 #endif
+
+// Dynamic shared memory beyond the default 48 KB needs the kernel's opt-in (a host-side attribute call, cheap next to the
+// launch; only rows of more than 512 dims ask for it)
+template <class K>
+static void allow_dynamic_smem(K kern, size_t bytes) {
+  if (bytes > 48 * 1024 - 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
 
 template <class R, int TK, bool DM, bool GEN>
 static int launch_gen(int kernel_id, const LaunchArgs& a) {
@@ -138,6 +146,24 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
         return 0;
       }
       break;
+    case K_GIST: {
+      auto kern = k_gist_transition<R, TK, DM, GEN>;
+      const size_t gsm = gist_smem_bytes<R, TK, DM>(a.P.D);
+      allow_dynamic_smem(kern, gsm);
+      kern<<<grid, block, gsm, st>>>(a.P, a.keys, a.q_in, a.logp_in, a.g_in, a.q_out, a.logp_out, a.g_out, a.gist);
+      return 0;
+    }
+    case K_GIST_CHAINS: {  // persistent grid, as K_NUTS_CHAINS
+      auto kern = k_gist_chains<R, TK, DM, GEN>;
+      int nb = 1;
+      const size_t gsm = gist_smem_bytes<R, TK, DM>(a.P.D);
+      allow_dynamic_smem(kern, gsm);
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kThreads, gsm) != cudaSuccess || nb < 1) nb = 1;
+      const long long want = ((long long)a.P.C + kWarpsPerBlock - 1) / kWarpsPerBlock;
+      const long long ctas = std::min<long long>(want, (long long)a.grid_override * nb);
+      kern<<<dim3((unsigned)ctas), block, gsm, st>>>(a.P, a.q_out, a.logp_out, a.g_out, a.gist);
+      return 0;
+    }
     case K_NUTS_CHAINS: {
       size_t sm_bytes = smem + (a.sample.ckpt_smem ? sizeof(float) * kWarpsPerBlock * 2 * a.sample.max_doublings * a.P.D : 0);
       // persistent grid: every CTA that fits (registers, checkpoint shared memory) on each of the grid_override SMs

@@ -368,11 +368,14 @@ template <class R>
 struct UserModelOf<R, TK_USER> { using type = bjx_user::Model<R>; };
 
 // Per-warp constant context: target scales and inverse mass held in registers for the whole kernel.
-template <class R, int TK, bool DM>
+// MSM: the diagonal inverse mass and the diagonal target's scales live in the warp's shared-memory rows msm and tsm (set
+// before init) instead of registers, for kernels that need those registers; the products are the same.
+template <class R, int TK, bool DM, bool MSM = false>
 struct Ctx {
   typename UserModelOf<R, TK>::type um;   // TK_USER: the user's model (its per-kernel state lives here)
-  float tw[(TK == TK_DIAG) ? R::NS : 1];  // target -1/s^2 (negated once: grad = q * tw, exactly -(q/s^2))
-  float mw[DM ? 1 : R::NS];               // diagonal inverse mass
+  float tw[(TK == TK_DIAG && !MSM) ? R::NS : 1];  // target -1/s^2 (negated once: grad = q * tw, exactly -(q/s^2))
+  float mw[(DM || MSM) ? 1 : R::NS];      // diagonal inverse mass
+  float *msm, *tsm;                       // MSM: the diagonal inverse mass and target rows in shared memory
   float* sm;                              // shared-memory slice (small dense paths)
   size_t moff;                            // small dense metric: offset of this chain's matrix (0 when shared)
   int lane;
@@ -380,14 +383,28 @@ struct Ctx {
   __device__ __forceinline__ void init(const Params& P, int chain, int lane_, float* sm_) {
     lane = lane_;
     sm = sm_;
-    if constexpr (TK == TK_DIAG) {
+    if constexpr (TK == TK_DIAG && MSM) {
+      float t[R::NS];
+      R::load_const(t, P.inv_var, P.D, lane);
+#pragma unroll
+      for (int s = 0; s < R::NS; ++s) t[s] = -t[s];
+      __syncwarp();
+      R::store_generic(t, tsm, P.D, lane);
+      __syncwarp();
+    } else if constexpr (TK == TK_DIAG) {
       R::load_const(tw, P.inv_var, P.D, lane);
 #pragma unroll
       for (int s = 0; s < R::NS; ++s) tw[s] = -tw[s];
     }
     if constexpr (TK == TK_USER) um.init(UserCtx{P.user, P.n_user, P.D, lane, sm});
     moff = 0;
-    if constexpr (!DM) R::load_const(mw, P.imm + (size_t)(chain / P.imm_group) * P.imm_stride, P.D, lane);
+    if constexpr (!DM && MSM) {
+      float t[R::NS];
+      R::load_const(t, P.imm + (size_t)(chain / P.imm_group) * P.imm_stride, P.D, lane);
+      __syncwarp();
+      R::store_generic(t, msm, P.D, lane);
+      __syncwarp();
+    } else if constexpr (!DM) R::load_const(mw, P.imm + (size_t)(chain / P.imm_group) * P.imm_stride, P.D, lane);
     else moff = (size_t)(chain / P.imm_group) * P.imm_stride;  // D*D per chain for per-chain dense metrics
   }
 
@@ -403,6 +420,9 @@ struct Ctx {
       } else if constexpr (R::NS <= 4) {  // small dense metrics exist for dim <= 128 only
         matvec_small<R>(P.imm + moff, p, v, sm, P.D, lane);
       }
+    } else if constexpr (MSM) {
+      R::load_generic(v, msm, P.D, lane);  // each lane reads back the slots it wrote
+      Vec<R::NS>::mul(v, v, p);
     } else {
       Vec<R::NS>::mul(v, mw, p);
     }
@@ -438,8 +458,17 @@ struct Ctx {
 #pragma unroll
         for (int s = 0; s < R::NS; ++s) d[s] = -d[s];
         Vec<R::NS>::add(d, q, d);
-        Vec<R::NS>::mul(g, d, tw);
+        if constexpr (MSM) {
+          R::load_generic(g, tsm, P.D, lane);
+          Vec<R::NS>::mul(g, d, g);
+        } else {
+          Vec<R::NS>::mul(g, d, tw);
+        }
         acc = WANT_LOGP ? Vec<R::NS>::dot_partial(d, g) : 0.f;
+      } else if constexpr (MSM) {
+        R::load_generic(g, tsm, P.D, lane);
+        Vec<R::NS>::mul(g, q, g);
+        acc = WANT_LOGP ? Vec<R::NS>::dot_partial(q, g) : 0.f;
       } else {
         Vec<R::NS>::mul(g, q, tw);
         acc = WANT_LOGP ? Vec<R::NS>::dot_partial(q, g) : 0.f;

@@ -164,6 +164,43 @@ def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_s
     return final, hist, acc, steps
 
 
+def sample_gist_native(rng_key, state, logdensity_fn, step_size, inverse_mass_matrix, num_steps, *,
+                       instance="trajectory_length", path_fraction=0.5, max_num_steps=1024, num_integration_steps=1,
+                       criterion="symmetric", max_search_steps=10, integrator=None, divergence_threshold=1000, thin=1,
+                       keep_history=True, chain_offset=0):
+    """``run_inference_algorithm`` for GIST without a Python-level loop (libbjx ``bjx_gist_sample``): one persistent
+    launch, same draws as ``num_steps`` calls of ``gist_trajectory_length`` (``instance="trajectory_length"``) or
+    ``gist_step_size`` (``instance="step_size"``, ``step_size`` being the initial step size) with the step keys
+    ``split(rng_key, T)[t]``.  Returns (final GISTState, positions [num_steps // thin, C, D] or None, acceptance rates
+    [num_steps, C], num_integration_steps int32 [num_steps, C])."""
+    from ._engine import get_engine
+    from ._lib import check, lib, ptr
+    from .mcmc import integrators
+    from .mcmc.composed import _seam, step_size as ss, trajectory_length as tl
+    if instance == "trajectory_length":
+        tuning = tl.tuning(path_fraction, max_num_steps)
+    elif instance == "step_size":
+        tuning = ss.tuning(num_integration_steps, criterion, max_search_steps)
+    else:
+        raise ValueError(f"instance must be 'trajectory_length' or 'step_size', got {instance!r}")
+    q, logp, g = (t.clone() for t in state)
+    eng = get_engine(q, logdensity_fn, divergence_threshold=divergence_threshold)
+    eng.set_integrator(integrators.as_coefficients(integrator or integrators.velocity_verlet))
+    eng.ensure_metric(inverse_mass_matrix)
+    key = rng_key.to(q.device).contiguous()
+    if key.ndim != 1:
+        raise ValueError("sample_gist_native takes ONE rng_key of shape [2]")
+    eng._key_mode(key, chain_offset)
+    C, D = q.shape
+    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
+    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    n_int = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    eps, eps_dev = eng._eps(step_size)
+    check(lib().bjx_gist_sample(eng.h, tuning.params, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev),
+                                int(num_steps), ptr(hist), int(thin), ptr(acc), ptr(n_int)), eng.h)
+    return _seam.GISTState(q, logp, g), hist, acc, n_int
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

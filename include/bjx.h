@@ -385,6 +385,60 @@ int bjx_adjusted_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q,
 int bjx_adjusted_mclmc_num_steps(bjx_handle_t h, int32_t steps_rule, const float* avg, int32_t min_steps,
                                  const uint32_t* random_generator_arg, int32_t* steps_out);
 
+/* ---- GIST: Gibbs self-tuning HMC (blackjax/mcmc/composed: gist_trajectory_length, gist_step_size) --------------------
+ * State (q [C,D], logp [C], grad [C,D]) as HMC's; initialise it with bjx_init_state.  One transition draws the momentum
+ * (key_momentum = split(key, 3)[0]), draws the tuning parameter given (q, p) (key_tuning = [1]), integrates, re-runs the
+ * same choice from the flipped proposal and accepts with uniform(key_accept = [2]) < exp(min(delta + log_ratio, 0)).
+ *   BJX_GIST_TRAJECTORY_LENGTH: U = steps until dot(q_n - q_0, p_n) < 0 or max_num_steps; L ~ randint(lo, U + 1) with
+ *     lo = max(1, floor(path_fraction * U)) in float32; the log ratio compares the widths of the forward and reverse
+ *     intervals, -inf when L is outside the reverse one (is_no_return_rejected).
+ *   BJX_GIST_STEP_SIZE: step size step_size * 2^j chosen by the doubling / halving search of at most max_search_steps + 1
+ *     trial trajectories of num_integration_steps steps (criterion BJX_GIST_SYMMETRIC or BJX_GIST_ASYMMETRIC); the
+ *     transition rejects unless the search from the proposal picks the same j and neither search was exhausted.
+ * Built on the warp-per-chain rows (dim <= 1024) with every row metric, target and integrator table there; dim > 1024 and
+ * the tensor-core dense path (a dense metric or dense Gaussian target beyond 128 dims) return BJX_E_UNSUPPORTED.  The
+ * handle keeps a scratch of 4 rows [C,D] (the initial momentum and the proposal) instead of the rollout, which is
+ * re-integrated: a transition costs about U + L + N gradient evaluations (trajectory length) or the trial steps of both
+ * searches plus num_integration_steps (step size). */
+#define BJX_GIST_TRAJECTORY_LENGTH 0
+#define BJX_GIST_STEP_SIZE 1
+#define BJX_GIST_SYMMETRIC 0
+#define BJX_GIST_ASYMMETRIC 1
+typedef struct {
+  int32_t instance;              /* BJX_GIST_TRAJECTORY_LENGTH or BJX_GIST_STEP_SIZE */
+  float path_fraction;           /* trajectory length: psi in [0, 1] (0.5) */
+  int32_t max_num_steps;         /* trajectory length: cap on each rollout, >= 1 (1024) */
+  int32_t num_integration_steps; /* step size: steps per trial and proposal trajectory, >= 1 (1) */
+  int32_t max_search_steps;      /* step size: >= 0 (10) */
+  int32_t criterion;             /* step size: BJX_GIST_SYMMETRIC (default) or BJX_GIST_ASYMMETRIC */
+} bjx_gist_params;
+/* Optional per-transition outputs (NULL => not written), [C] each unless marked. */
+typedef struct {
+  float* acceptance_rate;          /* exp(min(delta + log_ratio, 0)) */
+  uint8_t* is_accepted;
+  uint8_t* is_divergent;           /* -delta > divergence_threshold */
+  float* energy;                   /* energy of the proposal */
+  float* momentum;                 /* [C,D] momentum drawn at the start of the transition */
+  int32_t* num_integration_steps;  /* steps of the proposal's own trajectory (L, or num_integration_steps) */
+  int32_t* forward;                /* U (num_steps_to_uturn_forward) or j (step_index) */
+  int32_t* reverse;                /* N (num_steps_to_uturn_reverse) or j_rev (reverse_step_index) */
+  uint8_t* rejected;               /* is_no_return_rejected or search_exhausted */
+  float* a;                        /* step size: the thresholds (a, b) and the step size used */
+  float* b;
+  float* step_size;
+} bjx_gist_info;
+/* One transition; out may alias in (in place), step_size_dev [C] overrides step_size.  Keys follow bjx_set_key_mode. */
+int bjx_gist_step(bjx_handle_t h, const bjx_gist_params* params, const uint32_t* keys, const float* q_in,
+                  const float* logp_in, const float* grad_in, float* q_out, float* logp_out, float* grad_out,
+                  float step_size, const float* step_size_dev, const bjx_gist_info* info);
+/* run_inference_algorithm (util.py:150-213) for GIST, like bjx_nuts_sample: step keys = split(rng_key, num_steps), one
+ * persistent launch whose warps take whole chains through all transitions in place, bit-identical to num_steps calls of
+ * bjx_gist_step; no host synchronisation.  history (optional) float32 [num_steps / thin, C, D]; acceptance_history
+ * (optional) float32 [num_steps, C]; num_integration_steps_history (optional) int32 [num_steps, C]. */
+int bjx_gist_sample(bjx_handle_t h, const bjx_gist_params* params, const uint32_t* rng_key, float* q, float* logp,
+                    float* grad, float step_size, const float* step_size_dev, int32_t num_steps, float* history,
+                    int32_t thin, float* acceptance_history, int32_t* num_integration_steps_history);
+
 /* ---- Adjusted MCLMC tuning: adjusted_mclmc_find_L_and_step_size (blackjax/adaptation/adjusted_mclmc_adaptation.py:26-507)
  * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
  * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_adjusted_mclmc_step (BJX_E_UNSUPPORTED
