@@ -26,6 +26,9 @@ from .mcmc import adjusted_mclmc as _adjusted_mclmc
 from .mcmc import adjusted_mclmc_dynamic as _adjusted_mclmc_dynamic
 from .util import run_inference_algorithm, sample_hmc_native, sample_mclmc_native, sample_nuts_native  # noqa: F401
 from .util import sample_adjusted_mclmc_native, sample_gist_native  # noqa: F401
+from .util import sample_barker_native, sample_mala_native  # noqa: F401
+from .mcmc import barker as _barker
+from .mcmc import mala as _mala
 from .mcmc.composed import step_size as _gist_step_size
 from .mcmc.composed import trajectory_length as _gist_trajectory_length
 
@@ -55,5 +58,8 @@ gist_trajectory_length = GenerateSamplingAPI(_gist_trajectory_length.as_top_leve
                                              _gist_trajectory_length.init, _gist_trajectory_length.build_kernel)
 gist_step_size = GenerateSamplingAPI(_gist_step_size.as_top_level_api, _gist_step_size.init,  # blackjax/__init__.py:142
                                      _gist_step_size.build_kernel)
+mala = GenerateSamplingAPI(_mala.as_top_level_api, _mala.init, _mala.build_kernel)  # blackjax/__init__.py:120
+barker = GenerateSamplingAPI(_barker.as_top_level_api, _barker.init, _barker.build_kernel)  # blackjax/__init__.py:140
+barker_proposal = barker  # blackjax/__init__.py:141
 
 __version__ = "0.1.0"

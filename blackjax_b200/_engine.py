@@ -330,6 +330,28 @@ class Engine:
                                   ptr(go), eps, ptr(eps_dev), C.byref(info)), self.h)
         return qo, lo, go
 
+    def langevin_step(self, sampler, keys, q, logp, g, step_size, out=None, info_fields=None, chain_offset=0):
+        """One MALA (``sampler="mala"``, libbjx ``bjx_mala_step``) or Barker (``"barker"``, ``bjx_barker_step``)
+        transition; Barker uses the installed metric."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        g = _f32(g, (self.C, self.D), "logdensity_grad")
+        logp = _f32(logp, (self.C,), "logdensity")
+        qo, lo, go = out if out is not None else (torch.empty_like(q), torch.empty_like(logp), torch.empty_like(g))
+        eps, eps_dev = self._eps(step_size)
+        info = self._info(info_fields or {}, _lib.LangevinInfo)
+        fn = lib().bjx_mala_step if sampler == "mala" else lib().bjx_barker_step
+        check(fn(self.h, ptr(keys), ptr(q), ptr(logp), ptr(g), ptr(qo), ptr(lo), ptr(go), eps, ptr(eps_dev),
+                 C.byref(info)), self.h)
+        return qo, lo, go
+
+    def mala_step(self, keys, q, logp, g, step_size, out=None, info_fields=None, chain_offset=0):
+        return self.langevin_step("mala", keys, q, logp, g, step_size, out, info_fields, chain_offset)
+
+    def barker_step(self, keys, q, logp, g, step_size, out=None, info_fields=None, chain_offset=0):
+        return self.langevin_step("barker", keys, q, logp, g, step_size, out, info_fields, chain_offset)
+
     def adjusted_mclmc_num_steps(self, device_rule, avg, random_generator_arg):
         """The step counts int32 [C] of a dynamic rule ``device_rule = (rule, min_steps)`` at a per-chain ``avg`` [C]
         (libbjx ``bjx_adjusted_mclmc_num_steps``); random_generator_arg [C, 2] is read, not advanced.  The fixed rule

@@ -51,6 +51,11 @@ class GistInfo(C.Structure):
         "reverse", "rejected", "a", "b", "step_size")]
 
 
+class LangevinInfo(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("acceptance_rate", "is_accepted", "proposal_position", "proposal_logdensity",
+                                          "proposal_grad")]
+
+
 class LapsBurnInConfig(C.Structure):
     _fields_ = [("save_num", C.c_int32), ("alpha", C.c_float), ("C", C.c_float), ("r_end", C.c_float),
                 ("bias_type", C.c_int32), ("early_stop", C.c_int32), ("equi_full", C.c_int32)]
@@ -120,6 +125,14 @@ _SIGNATURES = {
                                 C.c_float, _f32p, C.POINTER(GistInfo)]),
     "bjx_gist_sample": (C.c_int, [C.c_void_p, C.POINTER(GistParams), _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
                                   C.c_int32, _f32p, C.c_int32, _f32p, C.c_void_p]),
+    "bjx_mala_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
+                                C.POINTER(LangevinInfo)]),
+    "bjx_barker_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p,
+                                  C.POINTER(LangevinInfo)]),
+    "bjx_mala_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, _f32p, C.c_int32,
+                                  _f32p]),
+    "bjx_barker_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, _f32p,
+                                    C.c_int32, _f32p]),
     "bjx_laps_state_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "bjx_laps_init": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32]),
     "bjx_laps_burn_in_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p,

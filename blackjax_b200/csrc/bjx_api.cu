@@ -54,7 +54,7 @@ int bjx_big_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
 // Execution path of a call (enum Route: bjx_internal.h).
 static Route rows_or_big(bjx_handle_t h) { return h->sc == SC_BIG ? ROUTE_BIG : ROUTE_ROWS; }
 // where the target alone is evaluated (bjx_init_state)
-static Route target_route(bjx_handle_t h) {
+Route target_route(bjx_handle_t h) {
   if (h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN && h->cfg.dim > 128) return ROUTE_DENSE;
   return rows_or_big(h);
 }
@@ -178,6 +178,7 @@ extern "C" int bjx_destroy(bjx_handle_t h) {
   if (h->gemm_ws) cudaFree(h->gemm_ws);
   if (h->sample_keys) cudaFree(h->sample_keys);
   if (h->gist_ws) cudaFree(h->gist_ws);
+  if (h->chol) cudaFree(h->chol);
   if (h->h_flag) cudaFreeHost(h->h_flag);
   delete h;
   return 0;
@@ -289,6 +290,13 @@ extern "C" int bjx_set_metric(bjx_handle_t h, int32_t kind, const float* imm) {
     for (int i = 0; i < D; ++i)
       for (int j = 0; j < D; ++j) m[(size_t)i * D + j] = (float)Li[(size_t)j * D + i];  // (L^-1)^T
     BJX_CUDA(cudaMemcpyAsync(h->msqrt, m.data(), m.size() * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    std::vector<float> l;
+    if (D <= 128) {  // L itself: M^-1/2 of Barker's proposal, which takes dense metrics on the row kernels only
+      l.resize((size_t)D * D);
+      for (size_t k = 0; k < l.size(); ++k) l[k] = (float)L[k];
+      if ((rc = bjx_grow(h, h->chol, h->chol_elems, elems, sizeof(float)))) return rc;
+      BJX_CUDA(cudaMemcpyAsync(h->chol, l.data(), l.size() * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    }
     BJX_CUDA(cudaStreamSynchronize(h->stream));
   } else if (kind == BJX_METRIC_DENSE_PER_CHAIN) {
     launch_chol_linv_t(C, D, imm, h->msqrt, h->stream);  // L^-T per chain on the device (float64)
@@ -388,8 +396,10 @@ Params make_params(bjx_handle_t h, float eps, const float* eps_dev) {
 
 int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, LaunchArgs& a) {
   a.stream = h->stream;
-  a.general_integrator = h->general_integrator;
-  const bool dm = h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK;
+  const bool langevin = kernel_id == K_LANGEVIN || kernel_id == K_LANGEVIN_CHAINS;
+  a.general_integrator = h->general_integrator && !langevin;  // MALA and Barker integrate nothing
+  const bool dm = (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK) &&
+                  !(langevin && a.langevin.kind == LANGEVIN_MALA);  // MALA has no metric
   int rc;
   const int tk = target_dependent ? h->cfg.target.kind : (int)BJX_TARGET_FUNNEL;
   switch (tk) {

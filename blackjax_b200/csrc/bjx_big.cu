@@ -370,3 +370,13 @@ int bjx_big_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
   a.q_out = q_out; a.logp_out = logp_out; a.g_out = g_out; a.n = L; a.info = info;
   return big_dispatch(h, BK_HMC, a);
 }
+// MALA / Barker on the big rows: one transition (A.step_keys == nullptr) or the native loop (bjx_langevin.cu)
+int bjx_big_langevin(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, const float* g_in,
+                     float* q_out, float* logp_out, float* g_out, float eps, const float* eps_dev, const LangevinArgs& A) {
+  BigLaunchArgs a{};
+  a.P = big_params(h, eps, eps_dev);
+  a.keys = keys; a.q_in = q_in; a.logp_in = logp_in; a.g_in = g_in;
+  a.q_out = q_out; a.logp_out = logp_out; a.g_out = g_out;
+  a.langevin = A;
+  return big_dispatch(h, BK_LANGEVIN, a);
+}

@@ -355,8 +355,125 @@ __global__ void __launch_bounds__(kBigThreads) k_big_hmc(BigParams P, const uint
   }
 }
 
+// MALA / Barker transitions (the warp kernels' langevin_transition_row, bjx_kernels.cuh) with a diagonal metric.  The
+// position and the proposal's (y, grad y), which the target addresses freely, sit in shared memory; the gradient at the
+// position is read from its [C, D] array where thread t uses elements t + 768 k (three rows fill the shared memory at
+// 18432 dims, and a fourth in registers spills).  One launch runs one transition (A.step_keys == nullptr: keys and
+// A.info as bjx_hmc_step's) or the A.num_steps transitions of the native loop, in place, with the position on chip
+// throughout and the gradient row rewritten on acceptance.
+template <int TK, int KIND>
+__global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const uint32_t* __restrict__ keys,
+                                                              const float* q_in, const float* logp_in, const float* g_in,
+                                                              float* q_out, float* logp_out, float* g_out, LangevinArgs A) {
+  extern __shared__ __align__(16) float sm[];
+  float *xs = sm, *y = sm + P.D, *gy = sm + 2 * (size_t)P.D, *red = sm + 3 * (size_t)P.D;
+  const int c = blockIdx.x, D = P.D, tid = threadIdx.x;
+  const size_t ro = (size_t)c * D;
+  __shared__ float langevin_slot[2];
+  const LangevinScalars sc = langevin_scalars(P.eps_dev ? P.eps_dev[c] : P.eps, langevin_slot,
+                                              KIND == LANGEVIN_MALA && tid == 0);
+  const float eps = sc.eps;
+  const float* ms = P.msqrt + (size_t)c * P.imm_stride;
+  const float* imm = P.imm + (size_t)c * P.imm_stride;
+  const bool loop = A.step_keys != nullptr;
+  const int T = loop ? A.num_steps : 1;
+  const float* gx = g_in + ro;  // the native loop: g_in == g_out, updated on acceptance
+  big_load(xs, q_in + ro, D);
+  float logp_x = logp_in[c];
+  bool acc = false;
+  __syncthreads();
+  for (int t = 0; t < T; ++t) {
+    // the transition's key, derived where each use needs it so that no key stays live across the target's evaluation
+    auto rng = [&]() {
+      const uint32_t* kt = loop ? A.step_keys + 2 * t : keys;
+      return P.key_shared ? fold_in(Key{kt[0], kt[1]}, P.chain_offset + (uint32_t)c) : Key{kt[2 * c], kt[2 * c + 1]};
+    };
+    float la, logp_y;  // log_p_accept; the proposal's log-density (the same in every thread)
+    if constexpr (KIND == LANGEVIN_MALA) {
+      const Key key_noise = fold_in(rng(), 0u);
+      for (int i = tid; i < D; i += kBigThreads)
+        y[i] = __fadd_rn(__fadd_rn(xs[i], __fmul_rn(eps, gx[i])), __fmul_rn(sc.s2(), normal_at(key_noise, (uint32_t)i)));
+      __syncthreads();
+      logp_y = big_value_and_grad<TK>(P, y, gy, red);
+      __syncthreads();
+      float sums[2] = {0.f, 0.f};
+      for (int i = tid; i < D; i += kBigThreads) {
+        const float tn = __fsub_rn(__fsub_rn(xs[i], y[i]), __fmul_rn(eps, gy[i]));
+        const float tp = __fsub_rn(__fsub_rn(y[i], xs[i]), __fmul_rn(eps, gx[i]));
+        sums[0] = __fmaf_rn(tn, tn, sums[0]);
+        sums[1] = __fmaf_rn(tp, tp, sums[1]);
+      }
+      block_sum<2>(sums, red);
+      la = safe_energy_diff(__fadd_rn(-logp_x, __fmul_rn(sc.w(), sums[1])), __fadd_rn(-logp_y, __fmul_rn(sc.w(), sums[0])));
+    } else {
+      const Key k0 = fold_in(rng(), 0u), key_normal = fold_in(k0, 0u), key_sign = fold_in(fold_in(k0, 1u), 0u);
+      for (int i = tid; i < D; i += kBigThreads) {
+        const float m = __ldg(ms + i);
+        const float z = __fmul_rn(eps, normal_at(key_normal, (uint32_t)i));
+        const float pb = expf(-log1pexp_naive(__fmul_rn(-__fmul_rn(m, gx[i]), z)));
+        const float bz = uniform01(key_sign, (uint32_t)i) < pb ? z : -z;
+        y[i] = __fadd_rn(xs[i], __fmul_rn(m, bz));
+      }
+      __syncthreads();
+      logp_y = big_value_and_grad<TK>(P, y, gy, red);
+      __syncthreads();
+      float sums[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int i = tid; i < D; i += kBigThreads) {
+        const float m = __ldg(ms + i), iv = __ldg(imm + i);
+        const float d = __fsub_rn(xs[i], y[i]);
+        const float v = __fmul_rn(iv, d), zt = __fmul_rn(sqrt_rn(iv), d);
+        sums[0] = __fmaf_rn(v, d, sums[0]);
+        sums[1] = __fmaf_rn(-v, -d, sums[1]);
+        sums[2] = __fadd_rn(sums[2], log1pexp_naive(__fmul_rn(-zt, __fmul_rn(m, gy[i]))));
+        sums[3] = __fadd_rn(sums[3], log1pexp_naive(__fmul_rn(zt, __fmul_rn(m, gx[i]))));
+      }
+      block_sum<4>(sums, red);
+      const float n = (float)D;
+      const float ratio = __fadd_rn(__fsub_rn(__fsub_rn(__fmul_rn(n, __fmul_rn(0.5f, sums[0])), sums[2]),
+                                              __fmul_rn(n, __fmul_rn(0.5f, sums[1]))),
+                                    sums[3]);
+      la = __fadd_rn(__fsub_rn(logp_y, logp_x), ratio);
+    }
+    const float p_acc = clip_max1(expf(la));
+    acc = uniform01(fold_in(rng(), 1u)) < p_acc;
+    if (!loop) {
+      if (A.info.proposal_position) big_store(A.info.proposal_position + ro, y, D);
+      if (A.info.proposal_grad) big_store(A.info.proposal_grad + ro, gy, D);
+    }
+    if (tid == 0) {
+      if (!loop) {
+        if (A.info.proposal_logdensity) A.info.proposal_logdensity[c] = logp_y;
+        if (A.info.acceptance_rate) A.info.acceptance_rate[c] = p_acc;
+        if (A.info.is_accepted) A.info.is_accepted[c] = acc;
+      } else if (A.acceptance_history) {
+        A.acceptance_history[(size_t)t * P.C + c] = p_acc;
+      }
+    }
+    if (acc) {  // each thread rewrites the elements it reads
+      for (int i = tid; i < D; i += kBigThreads) {
+        xs[i] = y[i];
+        g_out[ro + i] = gy[i];
+      }
+      logp_x = logp_y;
+    }
+    __syncthreads();
+    if (loop && A.history && ((t + 1) % A.thin) == 0)
+      big_store(A.history + ((size_t)((t + 1) / A.thin - 1) * P.C + c) * D, xs, D);
+  }
+  if (acc || loop) {
+    big_store(q_out + ro, xs, D);
+    if (tid == 0) logp_out[c] = logp_x;
+  } else if (q_out != q_in) {  // an out-of-place rejection carries the old state over
+    for (int i = tid; i < D / 4; i += kBigThreads) {
+      __stcs(reinterpret_cast<float4*>(q_out + ro) + i, __ldcs(reinterpret_cast<const float4*>(q_in + ro) + i));
+      __stcs(reinterpret_cast<float4*>(g_out + ro) + i, __ldcs(reinterpret_cast<const float4*>(g_in + ro) + i));
+    }
+    if (tid == 0) logp_out[c] = logp_x;
+  }
+}
+
 // ---- launch table shared by libbjx (built-in targets) and big-row plug-ins (TK = BJX_TARGET_USER) -------------------------
-enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2 };
+enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3 };
 struct BigLaunchArgs {
   BigParams P;
   const uint32_t* keys;
@@ -365,6 +482,7 @@ struct BigLaunchArgs {
   float* p_io;
   int n;                             // leapfrog steps | L
   InfoPtrs info;
+  LangevinArgs langevin;             // BK_LANGEVIN
   cudaStream_t stream;
 };
 
@@ -392,6 +510,12 @@ static int big_launch(int kernel_id, const BigLaunchArgs& a) {
       return go(k_big_leapfrog<TK, 24>, 2, a.P, a.q_out, a.p_io, a.logp_out, a.g_out, a.n);
     case BK_HMC:
       return go(k_big_hmc<TK>, 3, a.P, a.keys, a.q_in, a.logp_in, a.g_in, a.q_out, a.logp_out, a.g_out, a.n, a.info);
+    case BK_LANGEVIN:
+      if (a.langevin.kind == LANGEVIN_MALA)
+        return go(k_big_langevin<TK, LANGEVIN_MALA>, 3, a.P, a.keys, a.q_in, a.logp_in, a.g_in, a.q_out, a.logp_out,
+                  a.g_out, a.langevin);
+      return go(k_big_langevin<TK, LANGEVIN_BARKER>, 3, a.P, a.keys, a.q_in, a.logp_in, a.g_in, a.q_out, a.logp_out,
+                a.g_out, a.langevin);
     default:
       return (int)cudaErrorInvalidValue;
   }

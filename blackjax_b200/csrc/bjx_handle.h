@@ -26,6 +26,8 @@ struct bjx_handle_s {
   const float* imm = nullptr;    // caller-owned
   float* msqrt = nullptr;        // owned
   size_t msqrt_elems = 0;
+  float* chol = nullptr;         // owned: L = chol(M^-1) [D,D] of a dense metric (M^-1/2; Barker's proposal)
+  size_t chol_elems = 0;
   // NUTS workspace (owned, lazily allocated)
   bjx::NutsWs ws{};
   void* ws_block = nullptr;

@@ -63,6 +63,7 @@ struct LaunchArgs;
 // Gaussian target or a dense metric beyond 128 dims.
 enum Route { ROUTE_ROWS, ROUTE_BIG, ROUTE_DENSE };
 Route transition_route(bjx_handle_t h);                  // where a transition, which needs target and metric, runs
+Route target_route(bjx_handle_t h);                      // where a kernel that needs the target only runs
 bjx::Params make_params(bjx_handle_t h, float eps, const float* eps_dev);
 // launches kernel_id of the handle's (target, size class, metric, integrator) variant; target_dependent = false takes the
 // target-independent instance

@@ -11,7 +11,8 @@ namespace bjx {
 
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
 enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
-               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN, K_GIST, K_GIST_CHAINS };
+               K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN, K_GIST, K_GIST_CHAINS, K_LANGEVIN,
+               K_LANGEVIN_CHAINS };
 
 struct LaunchArgs {
   Params P;
@@ -25,6 +26,7 @@ struct LaunchArgs {
   AmclmcTuneArgs amclmc_tune;
   LapsArgs laps;
   GistArgs gist;
+  LangevinArgs langevin;
   int grid_override;   // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
@@ -83,6 +85,16 @@ struct Launcher {
 template <class K>
 static void allow_dynamic_smem(K kern, size_t bytes) {
   if (bytes > 48 * 1024 - 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+
+template <class R, int TK, bool DM, int KIND>
+static int launch_langevin(int kernel_id, const LaunchArgs& a, dim3 grid, size_t smem) {
+  if (kernel_id == K_LANGEVIN)
+    k_langevin_transition<R, TK, DM, KIND><<<grid, kThreads, smem, a.stream>>>(a.P, a.keys, a.q_in, a.logp_in, a.g_in,
+                                                                               a.q_out, a.logp_out, a.g_out, a.langevin);
+  else
+    k_langevin_chains<R, TK, DM, KIND><<<grid, kThreads, smem, a.stream>>>(a.P, a.q_out, a.logp_out, a.g_out, a.langevin);
+  return 0;
 }
 
 template <class R, int TK, bool DM, bool GEN>
@@ -164,6 +176,17 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
       kern<<<dim3((unsigned)ctas), block, gsm, st>>>(a.P, a.q_out, a.logp_out, a.g_out, a.gist);
       return 0;
     }
+    case K_LANGEVIN:
+    case K_LANGEVIN_CHAINS:
+      // velocity Verlet instances only (no integrator here); MALA has no metric (dispatched as diagonal), Barker's dense
+      // metric exists for dim <= 128
+      if constexpr (!GEN && !DM) {
+        if (a.langevin.kind == LANGEVIN_MALA) return launch_langevin<R, TK, DM, LANGEVIN_MALA>(kernel_id, a, grid, smem);
+        return launch_langevin<R, TK, DM, LANGEVIN_BARKER>(kernel_id, a, grid, smem);
+      } else if constexpr (!GEN && R::NS <= 4) {
+        if (a.langevin.kind == LANGEVIN_BARKER) return launch_langevin<R, TK, DM, LANGEVIN_BARKER>(kernel_id, a, grid, smem);
+      }
+      break;
     case K_NUTS_CHAINS: {
       size_t sm_bytes = smem + (a.sample.ckpt_smem ? sizeof(float) * kWarpsPerBlock * 2 * a.sample.max_doublings * a.P.D : 0);
       // persistent grid: every CTA that fits (registers, checkpoint shared memory) on each of the grid_override SMs

@@ -201,6 +201,51 @@ def sample_gist_native(rng_key, state, logdensity_fn, step_size, inverse_mass_ma
     return _seam.GISTState(q, logp, g), hist, acc, n_int
 
 
+def _sample_langevin_native(sampler, rng_key, state, logdensity_fn, step_size, num_steps, thin, keep_history,
+                            chain_offset, inverse_mass_matrix=None):
+    from ._engine import get_engine
+    from ._lib import check, lib, ptr
+    q, logp, g = (t.clone() for t in state)
+    eng = get_engine(q, logdensity_fn)
+    fn = lib().bjx_mala_sample
+    if sampler == "barker":
+        from .mcmc import barker
+        barker.install_metric(eng, inverse_mass_matrix)
+        fn = lib().bjx_barker_sample
+    key = rng_key.to(q.device).contiguous()
+    if key.ndim != 1:
+        raise ValueError(f"sample_{sampler}_native takes ONE rng_key of shape [2]")
+    eng._key_mode(key, chain_offset)
+    C, D = q.shape
+    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
+    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    eps, eps_dev = eng._eps(step_size)
+    check(fn(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev), int(num_steps), ptr(hist), int(thin),
+             ptr(acc)), eng.h)
+    return (q, logp, g), hist, acc
+
+
+def sample_mala_native(rng_key, state, logdensity_fn, step_size, num_steps, *, thin=1, keep_history=True,
+                       chain_offset=0):
+    """``run_inference_algorithm`` for MALA without a Python-level loop (libbjx ``bjx_mala_sample``): the same draws as
+    ``num_steps`` calls of ``mala`` with the step keys ``split(rng_key, T)[t]``.  Returns (final MALAState, positions
+    [num_steps // thin, C, D] or None, acceptance rates [num_steps, C])."""
+    from .mcmc.mala import MALAState
+    final, hist, acc = _sample_langevin_native("mala", rng_key, state, logdensity_fn, step_size, num_steps, thin,
+                                               keep_history, chain_offset)
+    return MALAState(*final), hist, acc
+
+
+def sample_barker_native(rng_key, state, logdensity_fn, step_size, num_steps, inverse_mass_matrix=None, *, thin=1,
+                         keep_history=True, chain_offset=0):
+    """``run_inference_algorithm`` for Barker's proposal without a Python-level loop (libbjx ``bjx_barker_sample``), as
+    ``sample_mala_native``; ``inverse_mass_matrix=None`` means ones."""
+    from .mcmc.barker import BarkerState
+    final, hist, acc = _sample_langevin_native("barker", rng_key, state, logdensity_fn, step_size, num_steps, thin,
+                                               keep_history, chain_offset, inverse_mass_matrix)
+    return BarkerState(*final), hist, acc
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

@@ -439,6 +439,45 @@ int bjx_gist_sample(bjx_handle_t h, const bjx_gist_params* params, const uint32_
                     float* grad, float step_size, const float* step_size_dev, int32_t num_steps, float* history,
                     int32_t thin, float* acceptance_history, int32_t* num_integration_steps_history);
 
+/* ---- MALA and Barker's proposal (blackjax/mcmc/mala.py, blackjax/mcmc/barker.py) ---------------------------------------
+ * State (q [C,D], logp [C], grad [C,D]) as HMC's; initialise it with bjx_init_state.  One transition is one gradient
+ * evaluation, a few passes over the row and one accept test: (k0, key_rmh) = split(key); accept when
+ * uniform(key_rmh) < clip(exp(log_p_accept), max=1).
+ *   MALA: y = x + step_size * grad + sqrt(2 step_size) * normal(k0, (D,)); log_p_accept = safe_energy_diff(E(y->x), E(x->y))
+ *     with E(a->b) = -logp_b + 0.25 (1 / step_size) |a - b - step_size grad_b|^2 (NaN -> -inf).  No metric: none needs to
+ *     be set, and a set one is ignored.
+ *   Barker: (key_normal, key_sign) = split(k0); z = step_size * normal(key_normal), c = (M^1/2)^T grad, sign +1 with
+ *     probability 1 / (1 + exp(-c z)) from uniform(split(key_sign, 1)[0], (D,)); y = x + M^1/2 (+-z); the acceptance
+ *     ratio of barker.py:80-128 as written there (a NaN ratio gives acceptance_rate NaN and a rejection).  Metrics:
+ *     BJX_METRIC_DIAG and BJX_METRIC_DIAG_PER_CHAIN for 1 <= dim <= 18432, BJX_METRIC_DENSE for dim <= 128 (M^1/2 =
+ *     chol(M^-1)^-T); other metrics return BJX_E_UNSUPPORTED.
+ * Rows: every row target and row plug-in for dim <= 1024, every big-row target and big plug-in for 1024 < dim <= 18432
+ * (dim % 4 == 0).  A dense Gaussian target beyond 128 dims (the tensor-core path) returns BJX_E_UNSUPPORTED. */
+typedef struct {                 /* optional per-transition outputs (NULL => not written) */
+  float* acceptance_rate;        /* [C]  clip(exp(log_p_accept), max=1) */
+  uint8_t* is_accepted;          /* [C] */
+  float* proposal_position;      /* [C,D] the proposal, accepted or not */
+  float* proposal_logdensity;    /* [C] */
+  float* proposal_grad;          /* [C,D] */
+} bjx_langevin_info;
+/* One transition; out may alias in (in place), step_size_dev [C] overrides step_size.  Keys follow bjx_set_key_mode. */
+int bjx_mala_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, const float* grad_in,
+                  float* q_out, float* logp_out, float* grad_out, float step_size, const float* step_size_dev,
+                  const bjx_langevin_info* info);
+int bjx_barker_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, const float* grad_in,
+                    float* q_out, float* logp_out, float* grad_out, float step_size, const float* step_size_dev,
+                    const bjx_langevin_info* info);
+/* run_inference_algorithm (util.py:150-213): step keys = split(rng_key, num_steps) on the device, then num_steps
+ * transitions in place with no host synchronisation, bit-identical to num_steps step calls with those keys (shared step
+ * key mode, bjx_set_key_mode's chain_offset honoured).  history (optional) float32 [num_steps / thin, C, D];
+ * acceptance_history (optional) float32 [num_steps, C]. */
+int bjx_mala_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, float* grad, float step_size,
+                    const float* step_size_dev, int32_t num_steps, float* history, int32_t thin,
+                    float* acceptance_history);
+int bjx_barker_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, float* grad, float step_size,
+                      const float* step_size_dev, int32_t num_steps, float* history, int32_t thin,
+                      float* acceptance_history);
+
 /* ---- Adjusted MCLMC tuning: adjusted_mclmc_find_L_and_step_size (blackjax/adaptation/adjusted_mclmc_adaptation.py:26-507)
  * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
  * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_adjusted_mclmc_step (BJX_E_UNSUPPORTED
