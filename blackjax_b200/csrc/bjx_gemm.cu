@@ -5,8 +5,9 @@
 //
 // Hand-written sm_90a kernel: persistent CTAs, one producer warp issuing TMA (cp.async.bulk.tensor) operand loads into
 // 128B-swizzled shared memory, two consumer warpgroups issuing wgmma.mma_async on them (each owns 64 rows of a 128 x 128
-// output tile, float32 accumulators in registers), a STAGES-deep mbarrier ring between them.  While the consumers run the
-// epilogue of one tile, the producer is already filling the ring for the next.
+// output tile, float32 accumulators in registers), a STAGES-deep mbarrier ring between them.  A consumer keeps a second
+// accumulator set: when a tile's K loop ends its sums move there, and its epilogue runs in slices under the next tile's
+// MMAs, one slice after each of the first K blocks is issued.
 //
 // float32 accuracy on the fp16 tensor-core path.  One TF32/BF16/FP16 MMA (11/8/11-bit significands) cannot meet the
 // 1e-5 parity tolerance, so every float32 operand is split into two binary16 terms x = x1 + x2 (+ a residual below
@@ -50,6 +51,11 @@ constexpr int kOffBar = kStages * kStageBytes;
 constexpr int kStgLd = kBN + 4;
 constexpr int kOffStg = kOffBar + 64;                      // after the 2 x kStages barriers, 16-byte aligned
 constexpr int kSmemBytes = kOffStg + 8 * 8 * kStgLd * 4 + 1024;  // + slack to align the base to 1024
+// A tile's epilogue runs in kSlices slices under the next tile's first kSlices K blocks (§3 of DESIGN.md: at D = 1024
+// one slice under each K block measured faster than 8 slices)
+constexpr int kSlices = 16;
+constexpr int kHalfSlices = kSlices / 2;  // per half of the accumulator fragment (8 rows of each consumer warp)
+static_assert(kSlices >= 2 && kSlices % 2 == 0 && kSlices <= 16, "whole halves, at most one staged row per slice");
 static_assert(kBN == kBM, "the operand tiles of X and A share one size");
 static_assert(kSmemBytes <= 232448, "over the 227 KB dynamic shared memory limit");
 
@@ -143,10 +149,16 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t u) { return __half22float2(
 //   warp 0, lane 0   TMA producer: four tiles per stage into the ring
 //   warpgroups 1-2   consumers: warpgroup w owns rows [64 (w-1), +64) of the tile; per stage 3 x 4 wgmma, and once
 //                    they are issued the previous stage's group is waited for and that stage released (one arrival per
-//                    consumer warp); per tile the epilogue from the registers, its global inputs loaded before the
-//                    tile's K loop, its rows of Y staged in shared memory beside the ring and stored row by row.  The
-//                    producer warpgroup runs on 40 registers per thread so that the consumers can hold those inputs
-//                    beside the accumulators (232).
+//                    consumer warp).  Then one slice of the PREVIOUS tile's epilogue runs from its saved accumulators
+//                    while this block's group is in flight: a half's rows of Y staged in shared memory beside the ring,
+//                    one staged row stored (Y and its two planes), or a half's row maxima recorded.  The epilogue's
+//                    global inputs are loaded during the K loop of its own tile, and the CTA's last tile runs its
+//                    epilogue whole after the loop.  The producer warpgroup runs on 40 registers per thread so that
+//                    the consumers can hold both accumulator sets and those inputs (232).
+// Slices and loads may run in any order relative to the tiles in flight: Y may alias Cin, but only elementwise (element
+// (r, c) is read as Cin and written as Y by the same thread, and no two tiles share an element), the planes a launch
+// writes are never the planes it reads (the momentum and position planes alternate between products), and the per-row
+// arrays read (step sizes, unscales, stale maxima) are never among the same launch's outputs.
 // Accumulator fragment of m64n128 (per warp of the warpgroup): d[4j + 2h + e] is row 16 warp + 8h + lane / 4,
 // column 8j + 2 (lane % 4) + e.
 __global__ void __launch_bounds__(kThreads, 1)
@@ -205,29 +217,56 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
   setmaxnreg_inc<232>();
   const int wg = (warp >> 2) - 1, wq = warp & 3;
   const float mat_unscale = E.mat_unscale ? E.mat_unscale[0] : 1.0f;
-  int s = 0;
+  float* stg = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + kOffStg) + (warp - 4) * 8 * kStgLd;
+
+  // One K block of the current tile: its MMAs are issued (k_issue) before the wait for block kb - 1's, whose stage is
+  // released only then (k_retire), so one wgmma group stays in flight.  wgmmas on one accumulator complete in issue
+  // order, so the sums are those of a serial loop.
+  float acc[64];
+  int s = 0, s_prev = 0;
   uint32_t ph = 0;
-  for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-    const int m0 = (t / tiles_n) * kBM, n0 = (t % tiles_n) * kBN;
-    // Every input of this tile's epilogue is loaded here, so that the loads complete behind the K loop's MMAs and the
-    // epilogue itself only computes and stores.  Y may alias Cin, but only elementwise: element (r, c) is read as Cin
-    // by one thread and written as Y only by a lane of the same warp, after that thread's Cin value went into it, so
-    // reading it before the K loop reads the same value.  The per-row arrays read here (step sizes, unscales, stale
-    // maxima) are never among the same launch's outputs.
-    float al_row[2], sc_row[2];
-    float2 cin[2][kBN / 8];
+  auto k_issue = [&]() {
+    mbar_wait(full_bar(s), ph);
+    const uint32_t st = base + (uint32_t)s * kStageBytes;
+    const uint32_t xo = (uint32_t)wg * (64u * kBK * 2u);  // this warpgroup's 64 rows of the X tiles
+    const uint64_t dx1 = wgmma_desc(st + xo), dx2 = wgmma_desc(st + kTileBytes + xo);
+    const uint64_t da1 = wgmma_desc(st + 2 * kTileBytes), da2 = wgmma_desc(st + 3 * kTileBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx1 + 2u * k, da1 + 2u * k);  // +32 bytes per K step
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx2 + 2u * k, da1 + 2u * k);
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx1 + 2u * k, da2 + 2u * k);
+    wgmma_commit();
+  };
+  auto k_retire = [&](const int kb) {
+    wgmma_wait<1>();
+    if (kb > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s_prev));
+    }
+    s_prev = s;
+    if (++s == kStages) { s = 0; ph ^= 1u; }
+  };
+
+  // The global inputs of the current tile's epilogue, loaded while its MMAs run: per row of the thread's two the step
+  // size, the activations' unscale and the stale maximum that chooses the lift (combined only once the tile's K loop
+  // is done, so that no instruction inside it waits for them), and the thread's 32 float2 of Cin.
+  float in_alpha[2], in_unscale[2], in_max[2];
+  float2 cin[2][kBN / 8];
+  auto load_inputs = [&](const int m0, const int n0) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = m0 + 64 * wg + 16 * wq + 8 * h + (lane >> 2);
-      // per-row epilogue factor and the lift of this row's planes
-      float al = E.alpha, sc = 1.0f;
+      in_alpha[h] = 1.0f;
+      in_unscale[h] = 1.0f;
+      in_max[h] = 0.0f;
       if (r < M) {
-        if (E.alpha_dev) al = E.alpha_dev[r] * E.alpha;
-        al = al * (E.x_unscale ? E.x_unscale[r] : 1.0f) * mat_unscale;
-        if (E.planes) sc = plane_lift(E.stale_max[r]);
+        if (E.alpha_dev) in_alpha[h] = E.alpha_dev[r];
+        if (E.x_unscale) in_unscale[h] = E.x_unscale[r];
+        if (E.planes) in_max[h] = E.stale_max[r];
       }
-      al_row[h] = al;
-      sc_row[h] = sc;
 #pragma unroll
       for (int j = 0; j < kBN / 8; ++j) {
         const int c = n0 + 8 * j + 2 * (lane & 3);
@@ -235,59 +274,35 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
         if (E.has_cin && r < M && c < N) cin[h][j] = *reinterpret_cast<const float2*>(Cin + (size_t)r * N + c);
       }
     }
+  };
 
-    // One wgmma group stays in flight: K block kb's MMAs are issued before the wait for block kb - 1's, whose stage is
-    // released only then.  wgmmas on one accumulator complete in issue order, so the sums are those of a serial loop.
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    int s_prev = 0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait(full_bar(s), ph);
-      const uint32_t st = base + (uint32_t)s * kStageBytes;
-      const uint32_t xo = (uint32_t)wg * (64u * kBK * 2u);  // this warpgroup's 64 rows of the X tiles
-      const uint64_t dx1 = wgmma_desc(st + xo), dx2 = wgmma_desc(st + kTileBytes + xo);
-      const uint64_t da1 = wgmma_desc(st + 2 * kTileBytes), da2 = wgmma_desc(st + 3 * kTileBytes);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx1 + 2u * k, da1 + 2u * k);  // +32 bytes per K step
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx2 + 2u * k, da1 + 2u * k);
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k) wgmma_m64n128k16(acc, dx1 + 2u * k, da2 + 2u * k);
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (kb > 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(s_prev));
-      }
-      s_prev = s;
-      if (++s == kStages) { s = 0; ph ^= 1u; }
-    }
-    wgmma_wait<0>();
-    fence_operands(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(empty_bar(s_prev));
+  // The finished tile whose epilogue is still to run: its accumulators, per-row epilogue factors and lifts, and origin.
+  float prev[64], pal[2] = {0.f, 0.f}, psc[2] = {1.f, 1.f};
+  int pm0 = 0, pn0 = 0;
+  bool pending = false;
+  float amax = 0.f;  // this thread's part of the current half's row maximum, from its staging to its atomicMax
 
-    // epilogue: two rows per thread, two adjacent columns per fragment register pair.  Y goes through this warp's
-    // staging rows in shared memory, so that every global store of the warp writes whole rows (a fragment store would
-    // touch 8 rows with 32 bytes each); the planes of Y are split from the staged rows, four columns per lane.
-    float* stg = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + kOffStg) + (warp - 4) * 8 * kStgLd;
+  // Slice e of that epilogue (two rows per thread, two adjacent columns per fragment register pair).  Y goes through
+  // this warp's staging rows in shared memory, so that every global store of the warp writes whole rows (a fragment
+  // store would touch 8 rows with 32 bytes each); the planes of Y are split from the staged rows, four columns per lane.
+  // Half h = e / kHalfSlices of the fragment is staged by its first slice, its 8 staged rows are stored over its
+  // kHalfSlices slices, and its last slice records the row maxima.
+  auto epilogue_slice = [&](const int e) {
+    const int h = e / kHalfSlices, j = e % kHalfSlices;
+    const int r0 = pm0 + 64 * wg + 16 * wq + 8 * h;  // the warp's 8 rows of this half
+    const int r = r0 + (lane >> 2);
+    const bool live = r < M;
+    if (j == 0) {
+      const float al = pal[h];
+      amax = 0.f;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r0 = m0 + 64 * wg + 16 * wq + 8 * h;  // the warp's 8 rows of this half
-      const int r = r0 + (lane >> 2);
-      const bool live = r < M;
-      const float al = al_row[h], sc = sc_row[h];
-      float amax = 0.f;
-#pragma unroll
-      for (int j = 0; j < kBN / 8; ++j) {
-        const int c = n0 + 8 * j + 2 * (lane & 3);
+      for (int jj = 0; jj < kBN / 8; ++jj) {
+        const int c = pn0 + 8 * jj + 2 * (lane & 3);
         if (!live || c >= N) continue;
-        const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+        const float a0 = prev[4 * jj + 2 * h], a1 = prev[4 * jj + 2 * h + 1];
         float2 y;
         if (E.has_cin) {
-          const float2 cv = cin[h][j];
+          const float2 cv = cin[h][jj];
           if (E.double_kick) {
             y.x = fmaf(al, a0, fmaf(al, a0, cv.x));
             y.y = fmaf(al, a1, fmaf(al, a1, cv.y));
@@ -298,27 +313,29 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
         } else {
           y = make_float2(al * a0, al * a1);
         }
-        *reinterpret_cast<float2*>(stg + (lane >> 2) * kStgLd + (c - n0)) = y;
+        *reinterpret_cast<float2*>(stg + (lane >> 2) * kStgLd + (c - pn0)) = y;
         if (E.planes) amax = fmaxf(amax, fmaxf(fabsf(y.x), fabsf(y.y)));
       }
       __syncwarp();
-      const int cw = n0 + 4 * lane;  // the four columns this lane stores of every staged row
+    }
+    const int cw = pn0 + 4 * lane;  // the four columns this lane stores of every staged row
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float sci = __shfl_sync(0xffffffffu, sc, 4 * i);
-        if (r0 + i >= M || cw >= N) continue;
-        const float4 y = *reinterpret_cast<const float4*>(stg + i * kStgLd + 4 * lane);
-        *reinterpret_cast<float4*>(Y + (size_t)(r0 + i) * N + cw) = y;
-        if (E.planes) {
-          const float s0 = y.x * sci, s1 = y.y * sci, s2 = y.z * sci, s3 = y.w * sci;
-          const uint32_t h01 = pack_h2(s0, s1), h23 = pack_h2(s2, s3);
-          const float2 f01 = unpack_h2(h01), f23 = unpack_h2(h23);
-          uint16_t* pri = planes_out + (size_t)(r0 + i) * 2 * KP_out + cw;
-          *reinterpret_cast<uint2*>(pri) = make_uint2(h01, h23);
-          *reinterpret_cast<uint2*>(pri + KP_out) =
-              make_uint2(pack_h2(s0 - f01.x, s1 - f01.y), pack_h2(s2 - f23.x, s3 - f23.y));
-        }
+    for (int i = 8 * j / kHalfSlices; i < 8 * (j + 1) / kHalfSlices; ++i) {
+      const float sci = __shfl_sync(0xffffffffu, psc[h], 4 * i);
+      if (r0 + i >= M || cw >= N) continue;
+      const float4 y = *reinterpret_cast<const float4*>(stg + i * kStgLd + 4 * lane);
+      *reinterpret_cast<float4*>(Y + (size_t)(r0 + i) * N + cw) = y;
+      if (E.planes) {
+        const float s0 = y.x * sci, s1 = y.y * sci, s2 = y.z * sci, s3 = y.w * sci;
+        const uint32_t h01 = pack_h2(s0, s1), h23 = pack_h2(s2, s3);
+        const float2 f01 = unpack_h2(h01), f23 = unpack_h2(h23);
+        uint16_t* pri = planes_out + (size_t)(r0 + i) * 2 * KP_out + cw;
+        *reinterpret_cast<uint2*>(pri) = make_uint2(h01, h23);
+        *reinterpret_cast<uint2*>(pri + KP_out) =
+            make_uint2(pack_h2(s0 - f01.x, s1 - f01.y), pack_h2(s2 - f23.x, s3 - f23.y));
       }
+    }
+    if (j == kHalfSlices - 1) {
       __syncwarp();  // the staging rows are rewritten by the next half
       if (E.planes) {  // the four lanes of a row hold its 128 columns of this tile
         amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
@@ -326,10 +343,60 @@ k_gemm_f16x3(const __grid_constant__ CUtensorMap tm_x,   // [K, 2, M]  binary16 
         if (live && (lane & 3) == 0) {
           atomicMax(reinterpret_cast<int*>(E.next_max) + r, __float_as_int(amax));
           E.zero_max[r] = 0.f;
-          if (n0 == 0) E.out_unscale[r] = 1.0f / sc;  // the tile of the first column block writes the lift
+          if (pn0 == 0) E.out_unscale[r] = 1.0f / psc[h];  // the tile of the first column block writes the lift
         }
       }
     }
+  };
+
+  for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const int m0 = (t / tiles_n) * kBM, n0 = (t % tiles_n) * kBN;
+    if (!pending) load_inputs(m0, n0);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    // The previous tile's epilogue runs under this tile's first kSlices K blocks, one slice behind each block's issue.
+    // Its Cin registers are free once its second half is staged, and this tile's inputs are loaded into them then.
+#pragma unroll
+    for (int e = 0; e < kSlices; ++e) {
+      if (e < nkb) k_issue();
+      if (e < nkb) k_retire(e);
+      if (pending) {
+        epilogue_slice(e);
+        if (e == kHalfSlices) load_inputs(m0, n0);
+      }
+    }
+    for (int kb = kSlices; kb < nkb; ++kb) {
+      k_issue();
+      k_retire(kb);
+    }
+    wgmma_wait<0>();
+    fence_operands(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_bar(s_prev));
+
+    // hand the tile over to the next tile's K loop
+#pragma unroll
+    for (int i = 0; i < 64; ++i) prev[i] = acc[i];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = m0 + 64 * wg + 16 * wq + 8 * h + (lane >> 2);
+      float al = E.alpha, sc = 1.0f;
+      if (r < M) {
+        if (E.alpha_dev) al = in_alpha[h] * E.alpha;
+        al = al * in_unscale[h] * mat_unscale;
+        if (E.planes) sc = plane_lift(in_max[h]);
+      }
+      pal[h] = al;
+      psc[h] = sc;
+    }
+    pm0 = m0;
+    pn0 = n0;
+    pending = true;
+  }
+  // the last tile's epilogue, whole
+  if (pending) {
+#pragma unroll
+    for (int e = 0; e < kSlices; ++e) epilogue_slice(e);
   }
 }
 
