@@ -14,6 +14,10 @@ The fixture tests/golden/gemm_f16x3_outputs.npz was recorded on an H100 80GB HBM
 stood before its epilogue loads were hoisted above the K loop and one wgmma group was kept in flight, by building that
 commit and running this file from its tree:
     python tests/test_gpu_gemm_bit_identity.py tests/golden/gemm_f16x3_outputs.npz
+
+These fixtures show that nothing changed, not that the output is right; correctness is checked independently by
+tests/test_gpu_gemm_probe.py (the kernel called directly, against float64 and bit-exact host models of every epilogue
+mode) and tests/test_gpu_dense_lift_window.py (the fused leapfrog at rows that leave the planes' exact lift window).
 """
 import hashlib
 import os

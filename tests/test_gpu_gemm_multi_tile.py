@@ -13,6 +13,10 @@ the per-row fingerprints of that file (a row digest, or a log-density as it is) 
 The fixture tests/golden/gemm_f16x3_multi_tile.npz holds the outputs of the kernel of commit 0a0c28c, whose epilogue ran
 after its tile's K loop, recorded on an H100 80GB HBM3 by running this file with the library built from that commit:
     python tests/test_gpu_gemm_multi_tile.py tests/golden/gemm_f16x3_multi_tile.npz
+
+These fixtures show that nothing changed, not that the output is right; correctness is checked independently by
+tests/test_gpu_gemm_probe.py (the kernel called directly, against float64 and bit-exact host models of every epilogue
+mode) and tests/test_gpu_dense_lift_window.py (the fused leapfrog at rows that leave the planes' exact lift window).
 """
 import hashlib
 import os

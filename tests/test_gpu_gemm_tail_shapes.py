@@ -11,6 +11,10 @@ Products, inputs and fingerprints are those of tests/test_gpu_gemm_bit_identity.
 The fixture tests/golden/gemm_f16x3_tail_shapes.npz was recorded on an H100 80GB HBM3 with the single-CTA kernel of
 commit 63c6297, by building that commit and running this file from its tree:
     python tests/test_gpu_gemm_tail_shapes.py tests/golden/gemm_f16x3_tail_shapes.npz
+
+These fixtures show that nothing changed, not that the output is right; correctness is checked independently by
+tests/test_gpu_gemm_probe.py (the kernel called directly, against float64 and bit-exact host models of every epilogue
+mode) and tests/test_gpu_dense_lift_window.py (the fused leapfrog at rows that leave the planes' exact lift window).
 """
 import os
 import sys
