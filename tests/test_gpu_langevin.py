@@ -1,6 +1,7 @@
 """MALA and Barker's proposal on the GPU: one teacher-forced transition against the float32 oracles (oracle/mala.py,
 oracle/barker.py) over the row size classes and the big rows, the native loops bit-identical to step calls, and the
-rejections.  Accept decisions and Barker's signs may differ from the oracle only where its margin is below 1e-5 * 64."""
+rejections.  Barker's signs may differ from the oracle only where its margin is below 1e-5 * 64, accept decisions only
+where u lies within that of the oracle's acceptance probability or between the two probabilities."""
 import numpy as np
 import pytest
 import torch
@@ -53,7 +54,12 @@ CASES = [("mala", "std", 1, "none"), ("mala", "diag", 18, "none"), ("mala", "fun
          ("mala", "diag", 1028, "none"),
          ("barker", "std", 2, "diag"), ("barker", "diag", 100, "per_chain"), ("barker", "funnel", 512, "diag"),
          ("barker", "diag", 128, "dense"), ("barker", "dense", 18, "dense"), ("barker", "diag", 1028, "diag"),
-         ("barker", "funnel", 2048, "per_chain"), ("barker", "std", 1024, "per_chain")]
+         ("barker", "funnel", 2048, "per_chain"), ("barker", "std", 1024, "per_chain"),
+         # the CTA rows past the 14-slot leapfrog edge and at the 3-row kernels' 18432 dims (221 664 B of shared memory)
+         ("mala", "diag", 10756, "none"), ("mala", "funnel", 18432, "none"),
+         ("barker", "funnel", 10756, "per_chain"), ("barker", "diag", 18432, "diag")]
+# the hierarchical logistic regression on the CTA rows: (D, through the hier_logit_big plug-in)
+HIER_LANGEVIN = [(10000, False), (18432, False), (18432, True)]
 
 
 def close_grad(a, b, kind, D):
@@ -85,12 +91,15 @@ def compare(sampler, keys, q, otgt, eps, imm, got, ginfo, D, kind):
     close_grad(ginfo["proposal_grad"][ok], gy[ok], kind, D)
     acc = ginfo["is_accepted"].astype(bool)
     same = acc == oi["is_accepted"]
-    assert np.all(same | (oi["margin"] <= TIE) | ~ok)
+    # p = exp(log_p_accept), a difference of sums whose terms are the size of the log-densities
+    close(ginfo["acceptance_rate"][ok], oi["acceptance_rate"][ok], scale=1.0 + np.abs(lq).max())
+    # a decision may differ only where u lies within TIE of the oracle's p or between the two p's (rows of ~1e4 dims have
+    # log-densities of ~1e4, whose rounding p carries)
+    dp = np.abs(ginfo["acceptance_rate"] - oi["acceptance_rate"])
+    assert np.all(same | (oi["margin"] <= np.maximum(TIE, dp)) | ~ok)
     keep = same & ok
     close(got[0][keep], oq[keep])
     close_grad(got[2][keep], og[keep], kind, D)
-    # p = exp(log_p_accept), a difference of sums whose terms are the size of the log-densities
-    close(ginfo["acceptance_rate"][keep], oi["acceptance_rate"][keep], scale=1.0 + np.abs(lq).max())
     return acc
 
 
@@ -103,6 +112,7 @@ def test_single_transition_matches_oracle(sampler, kind, D, metric, pce):
     q = start(kind, otgt, C, D, rs)
     base = (0.25 if sampler == "mala" else 1.2) * D ** (-1.0 / 3) * (0.4 if kind in ("diag", "dense") else 1.0)
     base *= 0.2 if (sampler == "mala" and kind == "diag") else 1.0
+    base *= 0.05 if (sampler == "mala" and kind == "funnel" and D > 10000) else 1.0   # the neck stiffens with D
     eps = (base * (0.5 + 0.5 * rs.uniform(size=C))).astype(F) if pce else F(base)
     imm = None
     if metric == "diag":
@@ -120,18 +130,25 @@ def test_single_transition_matches_oracle(sampler, kind, D, metric, pce):
 
 @pytest.mark.parametrize("sampler", ["mala", "barker"])
 def test_hier_logit_10000_matches_oracle(sampler):
-    """BASELINE config 5's hierarchical logistic regression on the CTA rows, teacher-forced."""
+    """BASELINE config 5's hierarchical logistic regression on the CTA rows, teacher-forced: at D = 10000, at the 3-row
+    kernels' 18432 dims, and there through the hier_logit_big plug-in."""
+    from blackjax_b200 import plugin
     from oracle import targets as otargets
-    D, C = 10000, 6
-    x, bits = bj.targets.HierLogit.synthetic_data(D - 4, seed=1)
-    tgt, otgt = bj.targets.HierLogit(x, bits), otargets.HierLogit(x, bits)
-    rs = np.random.default_rng(3)
-    q = (0.3 * rs.standard_normal((C, D))).astype(F)
-    imm = np.exp(rs.uniform(-0.3, 0.3, D)).astype(F) if sampler == "barker" else None
-    eps = F(2e-4) if sampler == "mala" else F(2e-3)
-    keys = oprng.split(oprng.key(4), C)
-    got, ginfo = run_step(sampler, tgt, q, float(eps), keys, None if imm is None else tf(imm))
-    compare(sampler, keys, q, otgt, eps, imm, got, ginfo, D, "hier")
+    C = 6
+    for D, user in HIER_LANGEVIN:
+        G = D - 4
+        x, bits = bj.targets.HierLogit.synthetic_data(G, seed=1)
+        tgt, otgt = bj.targets.HierLogit(x, bits), otargets.HierLogit(x, bits)
+        if user:
+            theta = np.concatenate([np.asarray([G, 0, 0, 0], F), x.reshape(-1).astype(F), bits.astype(F)])
+            tgt = bj.targets.UserTarget(D, plugin.read_example("hier_logit_big"), theta, name="hier_logit_big")
+        rs = np.random.default_rng(3)
+        q = (0.3 * rs.standard_normal((C, D))).astype(F)
+        imm = np.exp(rs.uniform(-0.3, 0.3, D)).astype(F) if sampler == "barker" else None
+        eps = F(2e-4) if sampler == "mala" else F(2e-3)
+        keys = oprng.split(oprng.key(4), C)
+        got, ginfo = run_step(sampler, tgt, q, float(eps), keys, None if imm is None else tf(imm))
+        compare(sampler, keys, q, otgt, eps, imm, got, ginfo, D, "hier")
 
 
 def stepwise(sampler, key, st, tgt, eps, imm, T_, thin, chain_offset):

@@ -691,94 +691,9 @@ def test_integrator_validation():
 
 
 # ---------------------------------------------------------------------------------------------------------
-# rows larger than a warp's registers (1024 < D <= 18432): CTA-per-chain kernels, incl. BASELINE config 5's target
+# rows larger than a warp's registers (1024 < D <= 18432): BASELINE config 5's target at full size (the kernels
+# against the oracle at every dispatch edge: tests/test_gpu_big_rows.py)
 # ---------------------------------------------------------------------------------------------------------
-def big_problem(kind, D, seed=41):
-    rs = np.random.default_rng(seed)
-    if kind == "diag":
-        s = np.exp(rs.uniform(-0.5, 0.5, D))
-        return T.DiagGaussian(s), otargets.DiagGaussian(s)
-    if kind == "funnel":
-        return T.Funnel(D), otargets.Funnel(D)
-    x, bits = T.HierLogit.synthetic_data(D - 4, seed=1)
-    return T.HierLogit(x, bits), otargets.HierLogit(x, bits)
-
-
-@pytest.mark.parametrize("kind, D, C", [("diag", 2048, 40), ("funnel", 1500, 24), ("hier", 1504, 24), ("hier", 10000, 6)])
-def test_big_rows_match_oracle(kind, D, C):
-    tgt, otgt = big_problem(kind, D)
-    rs = np.random.default_rng(5)
-    q = (0.3 * rs.standard_normal((C, D))).astype(F)
-    imm = np.exp(rs.uniform(-0.3, 0.3, D)).astype(F)
-    eng = _engine.Engine(DEV, C, D, tgt)
-    eng.set_metric(tf(imm))
-    om = ohmc.Metric(imm)
-    dq = tf(q)
-    logp, g = eng.init_state(dq)
-    lp0, g0 = otgt(q)
-    close(npy(g), g0, rtol=1e-5)
-    close(npy(logp), lp0, rtol=1e-5, scale=np.max(np.abs(lp0)) + 1)
-    keys = oprng.split(oprng.key(2), C)
-    p_ref = om.sample_momentum(keys, D)
-    close(npy(eng.sample_momentum(tk(keys))), p_ref, rtol=3e-6)
-    close(npy(eng.energy(tf(p_ref), logp)), -lp0 + om.kinetic_energy(p_ref), rtol=1e-5, scale=np.max(np.abs(lp0)) + D)
-    dp = tf(p_ref)
-    eps = F(0.01)
-    eng.leapfrog_(dq, dp, logp, g, float(eps), 5)
-    q1, p1, lp1, g1 = ohmc.static_integration(otgt, om, q, p_ref, lp0, g0, eps, 5)
-    close(npy(dq), q1, rtol=1e-5)
-    close(npy(dp), p1, rtol=2e-5)
-    close(npy(g), g1, rtol=2e-5)
-    close(npy(logp), lp1, rtol=1e-5, scale=np.max(np.abs(lp1)) + 1)
-    # one whole transition, teacher-forced
-    onew, oinfo = ohmc.hmc_kernel(keys, ohmc.init(q, otgt), otgt, eps, om, 6)
-    st = bj.hmc.init(tf(q), tgt)
-    new, info = bj.hmc.build_kernel(full_info=True)(tk(keys), st, tgt, float(eps), tf(imm), 6)
-    torch.cuda.synchronize()
-    close(npy(info.proposal.position), oinfo.proposal[0], rtol=1e-5)
-    close(npy(info.energy), oinfo.energy, rtol=1e-5, scale=np.max(np.abs(oinfo.energy)) + D)
-    u = oprng.uniform(oprng.split(keys, 2)[:, 1])
-    tie = np.abs(u - oinfo.acceptance_rate) < 1e-3
-    acc = npy(info.is_accepted)
-    assert ((acc == oinfo.is_accepted) | tie).all()
-    same = acc == oinfo.is_accepted
-    close(npy(new.position)[same], onew.position[same], rtol=1e-5)
-    with pytest.raises(bj.BjxError, match="dim <= 1024"):
-        bj.nuts.build_kernel()(tk(keys), st, tgt, 0.01, tf(imm), 3)
-
-
-@pytest.mark.parametrize("D, C, inplace", [(1504, 7, False), (1504, 1, True), (2052, 5, True)])
-def test_hier_logit_two_chains_per_cta_transition(D, C, inplace):
-    # k_big2_hmc_hier (two chains per CTA, momentum in registers): odd chain counts (the last CTA's second slot idles),
-    # per-chain step sizes and per-chain diagonal metrics, in place and out of place, against the oracle
-    tgt, otgt = big_problem("hier", D)
-    rs = np.random.default_rng(17)
-    q = (0.3 * rs.standard_normal((C, D))).astype(F)
-    imm = np.exp(rs.uniform(-0.3, 0.3, (C, D))).astype(F)
-    eps = (0.01 * np.exp(rs.uniform(-0.3, 0.3, C))).astype(F)
-    keys = oprng.split(oprng.key(3), C)
-    L = 5
-    onew, oinfo = ohmc.hmc_kernel(keys, ohmc.init(q, otgt), otgt, eps, oadapt._PerChainDiag(imm), L)
-    st = bj.hmc.init(tf(q), tgt)
-    q_before = st.position.clone()
-    new, info = bj.hmc.build_kernel(full_info=True, inplace=inplace)(tk(keys), st, tgt, tf(eps), tf(imm), L)
-    torch.cuda.synchronize()
-    close(npy(info.momentum), oinfo.momentum, rtol=3e-6)
-    close(npy(info.proposal.position), oinfo.proposal[0], rtol=1e-5)
-    close(npy(info.proposal.momentum), oinfo.proposal[1], rtol=2e-5)
-    close(npy(info.energy), oinfo.energy, rtol=1e-5, scale=np.max(np.abs(oinfo.energy)) + D)
-    close(npy(info.acceptance_rate), oinfo.acceptance_rate, rtol=2e-2, scale=1.0)
-    u = oprng.uniform(oprng.split(keys, 2)[:, 1])
-    acc = npy(info.is_accepted)
-    assert ((acc == oinfo.is_accepted) | (np.abs(u - oinfo.acceptance_rate) < 2e-2)).all()
-    same = acc == oinfo.is_accepted
-    close(npy(new.position)[same], onew.position[same], rtol=1e-5)
-    close(npy(new.logdensity_grad)[same], onew.logdensity_grad[same], rtol=2e-5)
-    close(npy(new.logdensity)[same], onew.logdensity[same], rtol=1e-5, scale=np.max(np.abs(onew.logdensity)) + 1)
-    rej = ~acc
-    assert torch.equal(new.position[torch.from_numpy(rej).to(DEV)], q_before[torch.from_numpy(rej).to(DEV)])
-
-
 def hier_logit_typical_start(C, D, device, seed=0):
     """A start in the typical set (the data-generating values + N(0, 0.7^2) group effects).  The origin is NOT usable:
     with every alpha_g == mu the log_tau gradient is -G, tau collapses and the centred model's funnel makes any
