@@ -2,6 +2,7 @@
 into the C ABI; all arrays are torch CUDA tensors used purely as device memory."""
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -351,6 +352,44 @@ class Engine:
 
     def barker_step(self, keys, q, logp, g, step_size, out=None, info_fields=None, chain_offset=0):
         return self.langevin_step("barker", keys, q, logp, g, step_size, out, info_fields, chain_offset)
+
+    def ensure_elliptical_prior(self, mean, cov):
+        """Install the elliptical slice prior N(mean, cov) (libbjx ``bjx_set_elliptical_prior``) unless this exact
+        content is installed: tensors are keyed as in ``ensure_metric``, a Python scalar mean by its value.  mean:
+        scalar or [D]; cov: [D] variances or [D, D]."""
+        def content_key(t):
+            if isinstance(t, torch.Tensor):
+                return (t.data_ptr(), tuple(t.shape), t._version, str(t.device))
+            return ("scalar", float(t)) if np.ndim(t) == 0 else None
+        key = (content_key(mean), content_key(cov))
+        given = (mean, cov)
+        if None not in key and key == getattr(self, "_prior_key", None):
+            return
+        mean = torch.as_tensor(mean, dtype=torch.float32, device=self.device)
+        cov = torch.as_tensor(cov, dtype=torch.float32, device=self.device)
+        if cov.ndim == 1 and cov.shape[0] == self.D:
+            kind = _lib.METRIC_DIAG
+        elif cov.ndim == 2 and tuple(cov.shape) == (self.D, self.D):
+            kind = _lib.METRIC_DENSE
+        else:
+            raise ValueError(f"cov has shape {tuple(cov.shape)}, expected ({self.D},) or ({self.D}, {self.D})")
+        m = torch.broadcast_to(mean, (self.D,)).contiguous()
+        cov = cov.contiguous()
+        check(lib().bjx_set_elliptical_prior(self.h, kind, ptr(m), ptr(cov)), self.h)
+        self._prior = given  # the key's tensors stay alive, so their addresses are not reused
+        self._prior_key = key if None not in key else None
+
+    def elliptical_slice_step(self, keys, q, logl, max_subiter, out=None, info_fields=None, chain_offset=0):
+        """One elliptical slice transition (libbjx ``bjx_elliptical_slice_step``) under the installed prior."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        logl = _f32(logl, (self.C,), "logdensity")
+        qo, lo = out if out is not None else (torch.empty_like(q), torch.empty_like(logl))
+        info = self._info(info_fields or {}, _lib.EllipticalSliceInfo)
+        check(lib().bjx_elliptical_slice_step(self.h, ptr(keys), ptr(q), ptr(logl), ptr(qo), ptr(lo), int(max_subiter),
+                                              C.byref(info)), self.h)
+        return qo, lo
 
     def adjusted_mclmc_num_steps(self, device_rule, avg, random_generator_arg):
         """The step counts int32 [C] of a dynamic rule ``device_rule = (rule, min_steps)`` at a per-chain ``avg`` [C]

@@ -56,6 +56,10 @@ class LangevinInfo(C.Structure):
                                           "proposal_grad")]
 
 
+class EllipticalSliceInfo(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("momentum", "theta", "subiter", "exhausted")]
+
+
 class LapsBurnInConfig(C.Structure):
     _fields_ = [("save_num", C.c_int32), ("alpha", C.c_float), ("C", C.c_float), ("r_end", C.c_float),
                 ("bias_type", C.c_int32), ("early_stop", C.c_int32), ("equi_full", C.c_int32)]
@@ -133,6 +137,11 @@ _SIGNATURES = {
                                   _f32p]),
     "bjx_barker_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, C.c_float, _f32p, C.c_int32, _f32p,
                                     C.c_int32, _f32p]),
+    "bjx_set_elliptical_prior": (C.c_int, [C.c_void_p, C.c_int32, _f32p, _f32p]),
+    "bjx_elliptical_slice_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32,
+                                            C.POINTER(EllipticalSliceInfo)]),
+    "bjx_elliptical_slice_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, _f32p, C.c_int32,
+                                              C.c_void_p]),
     "bjx_laps_state_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "bjx_laps_init": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32]),
     "bjx_laps_burn_in_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p,

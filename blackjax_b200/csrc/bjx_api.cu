@@ -179,6 +179,8 @@ extern "C" int bjx_destroy(bjx_handle_t h) {
   if (h->sample_keys) cudaFree(h->sample_keys);
   if (h->gist_ws) cudaFree(h->gist_ws);
   if (h->chol) cudaFree(h->chol);
+  if (h->ess_prior) cudaFree(h->ess_prior);
+  if (h->ess_ws) cudaFree(h->ess_ws);
   if (h->h_flag) cudaFreeHost(h->h_flag);
   delete h;
   return 0;
@@ -245,6 +247,21 @@ extern "C" int bjx_synchronize(bjx_handle_t h) {
   return 0;
 }
 
+bool cholesky_f64(const std::vector<float>& a, int D, std::vector<double>& L) {
+  L.assign((size_t)D * D, 0.0);
+  for (int i = 0; i < D; ++i)
+    for (int j = 0; j <= i; ++j) {
+      double s = a[(size_t)i * D + j];
+      for (int k = 0; k < j; ++k) s -= L[(size_t)i * D + k] * L[(size_t)j * D + k];
+      if (i == j) {
+        if (!(s > 0.0)) return false;
+        L[(size_t)i * D + i] = sqrt(s);
+      } else
+        L[(size_t)i * D + j] = s / L[(size_t)j * D + j];
+    }
+  return true;
+}
+
 extern "C" int bjx_set_metric(bjx_handle_t h, int32_t kind, const float* imm) {
   if (!h || !imm) return bjx_fail(h, BJX_E_INVALID, "null argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
@@ -268,17 +285,8 @@ extern "C" int bjx_set_metric(bjx_handle_t h, int32_t kind, const float* imm) {
     std::vector<float> a((size_t)D * D);
     BJX_CUDA(cudaMemcpyAsync(a.data(), imm, a.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     BJX_CUDA(cudaStreamSynchronize(h->stream));
-    std::vector<double> L((size_t)D * D, 0.0), Li((size_t)D * D, 0.0);
-    for (int i = 0; i < D; ++i)
-      for (int j = 0; j <= i; ++j) {
-        double s = a[(size_t)i * D + j];
-        for (int k = 0; k < j; ++k) s -= L[(size_t)i * D + k] * L[(size_t)j * D + k];
-        if (i == j) {
-          if (!(s > 0.0)) return bjx_fail(h, BJX_E_INVALID, "inverse mass matrix is not positive definite");
-          L[(size_t)i * D + i] = sqrt(s);
-        } else
-          L[(size_t)i * D + j] = s / L[(size_t)j * D + j];
-      }
+    std::vector<double> L, Li((size_t)D * D, 0.0);
+    if (!cholesky_f64(a, D, L)) return bjx_fail(h, BJX_E_INVALID, "inverse mass matrix is not positive definite");
     for (int c = 0; c < D; ++c) {  // Li = L^-1 by forward substitution, column c
       for (int i = c; i < D; ++i) {
         double s = (i == c) ? 1.0 : 0.0;
@@ -397,9 +405,12 @@ Params make_params(bjx_handle_t h, float eps, const float* eps_dev) {
 int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, LaunchArgs& a) {
   a.stream = h->stream;
   const bool langevin = kernel_id == K_LANGEVIN || kernel_id == K_LANGEVIN_CHAINS;
-  a.general_integrator = h->general_integrator && !langevin;  // MALA and Barker integrate nothing
-  const bool dm = (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK) &&
-                  !(langevin && a.langevin.kind == LANGEVIN_MALA);  // MALA has no metric
+  const bool ess = kernel_id == K_ESS || kernel_id == K_ESS_CHAINS;
+  a.general_integrator = h->general_integrator && !langevin && !ess;  // MALA, Barker and elliptical slice integrate nothing
+  // elliptical slice has no metric: its dense variant is the small dense prior's
+  const bool dm = ess ? a.ess.prior == ESS_PRIOR_DENSE
+                      : (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK) &&
+                            !(langevin && a.langevin.kind == LANGEVIN_MALA);  // MALA has no metric
   int rc;
   const int tk = target_dependent ? h->cfg.target.kind : (int)BJX_TARGET_FUNNEL;
   switch (tk) {

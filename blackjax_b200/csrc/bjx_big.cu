@@ -380,3 +380,13 @@ int bjx_big_langevin(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
   a.langevin = A;
   return big_dispatch(h, BK_LANGEVIN, a);
 }
+// Elliptical slice sampling on the big rows: one transition (A.step_keys == nullptr) or the native loop (bjx_ess.cu)
+int bjx_big_ess(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logl_in, float* q_out,
+                float* logl_out, const EssArgs& A) {
+  BigLaunchArgs a{};
+  a.P = big_params(h, 0.f, nullptr);
+  a.keys = keys; a.q_in = q_in; a.logp_in = logl_in;
+  a.q_out = q_out; a.logp_out = logl_out;
+  a.ess = A;
+  return big_dispatch(h, BK_ESS, a);
+}

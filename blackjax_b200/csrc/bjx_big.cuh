@@ -472,8 +472,85 @@ __global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const
   }
 }
 
+// Elliptical slice transitions (the warp kernels' ess_transition_row, bjx_kernels.cuh) with a diagonal prior.  The
+// proposal and its gradient scratch, which the target addresses freely, sit in shared memory; x and nu are read from
+// global memory on every sub-iteration (nu from the [C, D] scratch A.nu), each thread using the elements t + 768 k that
+// it writes itself: a third row of 18432 floats does not fit beside them.  One launch runs one transition (A.step_keys ==
+// nullptr: keys and A.info as bjx_elliptical_slice_step's) or the A.num_steps transitions of the native loop in place.
+template <int TK>
+__global__ void __launch_bounds__(kBigThreads) k_big_ess(BigParams P, const uint32_t* __restrict__ keys, const float* q_in,
+                                                         const float* logl_in, float* q_out, float* logl_out, EssArgs A) {
+  extern __shared__ __align__(16) float sm[];
+  float *p = sm, *g = sm + P.D, *red = sm + 2 * (size_t)P.D;
+  const int c = blockIdx.x, D = P.D, tid = threadIdx.x;
+  const size_t ro = (size_t)c * D;
+  const bool loop = A.step_keys != nullptr;
+  const int T = loop ? A.num_steps : 1;
+  const float* x = q_in + ro;  // the native loop: q_in == q_out, rewritten on acceptance
+  float* nu = A.nu + ro;
+  float logl_x = logl_in[c];
+  for (int t = 0; t < T; ++t) {
+    auto rng = [&]() {
+      const uint32_t* kt = loop ? A.step_keys + 2 * t : keys;
+      return P.key_shared ? fold_in(Key{kt[0], kt[1]}, P.chain_offset + (uint32_t)c) : Key{kt[2 * c], kt[2 * c + 1]};
+    };
+    {
+      const Key key_momentum = fold_in(rng(), 1u);
+      for (int i = tid; i < D; i += kBigThreads)
+        nu[i] = __fadd_rn(__ldg(A.mean + i), __fmul_rn(__ldg(A.scale + i), normal_at(key_momentum, (uint32_t)i)));
+    }
+    const float logy = __fadd_rn(logl_x, logf(uniform01(fold_in(rng(), 2u))));
+    float theta = __fmul_rn(kEssTwoPi, uniform01(fold_in(rng(), 3u)));
+    float theta_min = __fsub_rn(theta, kEssTwoPi), theta_max = theta;
+    float sn, cs;
+    auto propose = [&]() {
+      ess_sincos(theta, sn, cs);
+      for (int i = tid; i < D; i += kBigThreads) p[i] = ess_point(x[i], nu[i], __ldg(A.mean + i), cs, sn);
+      __syncthreads();
+      const float l = big_value_and_grad<TK>(P, p, g, red);
+      __syncthreads();
+      return l;
+    };
+    float logl_p = propose();
+    int subiter = 1;
+    while (logl_p <= logy && subiter < A.max_subiter) {
+      const float f = uniform01(fold_in(fold_in(rng(), 0u), (uint32_t)subiter));
+      theta = fmaxf(theta_min, __fadd_rn(__fmul_rn(f, __fsub_rn(theta_max, theta_min)), theta_min));
+      logl_p = propose();
+      if (theta < 0.f) theta_min = theta;
+      if (theta > 0.f) theta_max = theta;
+      ++subiter;
+    }
+    const bool exhausted = logl_p <= logy;
+    if (!loop) {
+      if (A.info.momentum)
+        for (int i = tid; i < D; i += kBigThreads)
+          A.info.momentum[ro + i] = exhausted ? nu[i] : ess_point(nu[i], x[i], __ldg(A.mean + i), cs, -sn);
+      if (tid == 0) {
+        if (A.info.theta) A.info.theta[c] = exhausted ? 0.f : theta;
+        if (A.info.subiter) A.info.subiter[c] = subiter;
+        if (A.info.exhausted) A.info.exhausted[c] = exhausted;
+      }
+    } else if (tid == 0 && A.subiter_history) {
+      A.subiter_history[(size_t)t * P.C + c] = subiter;
+    }
+    if (!exhausted) {  // each thread rewrites the elements it reads
+      for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = p[i];
+      logl_x = logl_p;
+      x = q_out + ro;
+    } else if (q_out != q_in) {  // an out-of-place call carries the old state over
+      for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = x[i];
+    }
+    if (loop && A.history && ((t + 1) % A.thin) == 0) {
+      float* hrow = A.history + ((size_t)((t + 1) / A.thin - 1) * P.C + c) * D;
+      for (int i = tid; i < D; i += kBigThreads) hrow[i] = x[i];
+    }
+  }
+  if (tid == 0) logl_out[c] = logl_x;
+}
+
 // ---- launch table shared by libbjx (built-in targets) and big-row plug-ins (TK = BJX_TARGET_USER) -------------------------
-enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3 };
+enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3, BK_ESS = 4 };
 struct BigLaunchArgs {
   BigParams P;
   const uint32_t* keys;
@@ -483,6 +560,7 @@ struct BigLaunchArgs {
   int n;                             // leapfrog steps | L
   InfoPtrs info;
   LangevinArgs langevin;             // BK_LANGEVIN
+  EssArgs ess;                       // BK_ESS: q_in, logp_in (logL), q_out, logp_out
   cudaStream_t stream;
 };
 
@@ -516,6 +594,8 @@ static int big_launch(int kernel_id, const BigLaunchArgs& a) {
                   a.g_out, a.langevin);
       return go(k_big_langevin<TK, LANGEVIN_BARKER>, 3, a.P, a.keys, a.q_in, a.logp_in, a.g_in, a.q_out, a.logp_out,
                 a.g_out, a.langevin);
+    case BK_ESS:
+      return go(k_big_ess<TK>, 2, a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.ess);
     default:
       return (int)cudaErrorInvalidValue;
   }

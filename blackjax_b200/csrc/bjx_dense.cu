@@ -161,8 +161,9 @@ __global__ void k_rows_open(int C, int D, float* __restrict__ p, const float* __
   }
 }
 
-// z[c, i] = normal(key_c, (D,))[i] with key_c = split(rng_key_c, 2)[0] when split_first (hmc.py:299,302 -> util.py:89-91)
-__global__ void k_dense_normal(int C, int D, const uint32_t* __restrict__ keys, float* __restrict__ z, bool split_first,
+// z[c, i] = normal(key_c, (D,))[i] with key_c = split(rng_key_c, n)[sub] when sub >= 0 (hmc.py:299,302 -> util.py:89-91:
+// sub = 0; elliptical_slice.py:205: sub = 1), the chain's key itself when sub < 0
+__global__ void k_dense_normal(int C, int D, const uint32_t* __restrict__ keys, float* __restrict__ z, int sub,
                                int key_shared, uint32_t chain_offset) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long n4 = (long long)C * D / 4;
@@ -171,7 +172,7 @@ __global__ void k_dense_normal(int C, int D, const uint32_t* __restrict__ keys, 
   const int c = (int)(e / D);
   const uint32_t i = (uint32_t)(e % D);
   Key km = key_shared ? fold_in(Key{keys[0], keys[1]}, chain_offset + (uint32_t)c) : Key{keys[2 * c], keys[2 * c + 1]};
-  if (split_first) km = fold_in(km, 0u);
+  if (sub >= 0) km = fold_in(km, (uint32_t)sub);
   float4 o;
   o.x = normal_at(km, i);
   o.y = normal_at(km, i + 1);
@@ -331,10 +332,10 @@ struct DenseWs {
   uint16_t* xs[2];     // [C, 2, KP] binary16 operand planes of the momentum (PL_P) and position (PL_Q) rows
   float* unscale[2];   // [C] 2^-s_r of those planes
   float* rmax[2];      // [3, C] row maxima of p / q: previous production, current accumulator, next (cleared)
-  float* mat_max;      // [3] max |a| of the constant matrices
-  float* mat_unscale;  // [3] 2^-s_A
+  float* mat_max;      // [4] max |a| of the constant matrices
+  float* mat_unscale;  // [4] 2^-s_A
 };
-enum { MAT_IMM = 0, MAT_MSQRT = 1, MAT_PREC = 2 };
+enum { MAT_IMM = 0, MAT_MSQRT = 1, MAT_PREC = 2, MAT_PRIOR = 3 };
 enum { PL_P = 0, PL_Q = 1 };
 
 // Every helper below works on the first n rows of its [C, D] / [C] arrays, all on the handle's stream: n = C, except for
@@ -346,7 +347,7 @@ static int dense_ws(bjx_handle_t h, DenseWs& w) {
   const size_t KP = plane_stride((int)D);
   const size_t xsb = ((C * 2 * KP * sizeof(uint16_t)) + 255) & ~(size_t)255;
   const size_t mat = ((D * 2 * KP * sizeof(uint16_t)) + 255) & ~(size_t)255;
-  const size_t need = 4 * row + 11 * vec + 2 * xsb + 3 * mat + 256;
+  const size_t need = 4 * row + 11 * vec + 2 * xsb + 4 * mat + 256;
   int rc = bjx_grow(h, h->dense_block, h->dense_bytes, need, 1);
   if (rc) return rc;
   char* b = (char*)h->dense_block;
@@ -357,19 +358,21 @@ static int dense_ws(bjx_handle_t h, DenseWs& w) {
   w.rmax[PL_P] = (float*)(vb + 5 * vec); w.rmax[PL_Q] = (float*)(vb + 8 * vec);  // 3 x vec each
   char* xb = vb + 11 * vec;
   w.xs[PL_P] = (uint16_t*)xb; w.xs[PL_Q] = (uint16_t*)(xb + xsb);
-  for (int m = 0; m < 3; ++m) h->dense_mat_s[m] = (uint16_t*)(xb + 2 * xsb + m * mat);
-  w.mat_max = (float*)(xb + 2 * xsb + 3 * mat);
+  for (int m = 0; m < 4; ++m) h->dense_mat_s[m] = (uint16_t*)(xb + 2 * xsb + m * mat);
+  w.mat_max = (float*)(xb + 2 * xsb + 4 * mat);
   w.mat_unscale = w.mat_max + 4;
   if (h->dense_bytes_built != need) {  // fresh block: zero the plane pads, every split matrix must be rebuilt
-    BJX_CUDA(cudaMemsetAsync(vb, 0, 11 * vec + 2 * xsb + 3 * mat, h->stream));
-    for (int m = 0; m < 3; ++m) h->dense_mat_src[m] = nullptr;
+    BJX_CUDA(cudaMemsetAsync(vb, 0, 11 * vec + 2 * xsb + 4 * mat, h->stream));
+    for (int m = 0; m < 4; ++m) h->dense_mat_src[m] = nullptr;
     h->dense_bytes_built = need;
   }
-  // (re)build the split copies of the constant matrices whose source changed (set_metric / set_target)
-  const float* src[3] = {h->metric_kind == BJX_METRIC_DENSE ? h->imm : nullptr,
+  // (re)build the split copies of the constant matrices whose source changed (set_metric / set_target /
+  // set_elliptical_prior)
+  const float* src[4] = {h->metric_kind == BJX_METRIC_DENSE ? h->imm : nullptr,
                          h->metric_kind == BJX_METRIC_DENSE ? h->msqrt : nullptr,
-                         h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN ? h->cfg.target.precision : nullptr};
-  for (int m = 0; m < 3; ++m) {
+                         h->cfg.target.kind == BJX_TARGET_DENSE_GAUSSIAN ? h->cfg.target.precision : nullptr,
+                         h->ess_kind == BJX_METRIC_DENSE ? h->ess_prior + h->cfg.dim : nullptr};
+  for (int m = 0; m < 4; ++m) {
     if (src[m] && (h->dense_mat_src[m] != src[m] || h->dense_mat_ver[m] != h->dense_version)) {
       BJX_CUDA(cudaMemsetAsync(w.mat_max + m, 0, sizeof(float), h->stream));
       k_absmax<<<sm_count(), 256, 0, h->stream>>>((long long)D * D / 4, src[m], w.mat_max + m);
@@ -483,7 +486,8 @@ static int dense_momentum(bjx_handle_t h, DenseWs& w, int n, const uint32_t* key
   const int D = h->cfg.dim;
   const bool dense_m = (h->metric_kind == BJX_METRIC_DENSE);
   float* z = dense_m ? w.v : p_out;
-  k_dense_normal<<<g4((long long)n * D / 4), 256, 0, h->stream>>>(n, D, keys, z, split_first, h->key_shared, h->chain_offset);
+  k_dense_normal<<<g4((long long)n * D / 4), 256, 0, h->stream>>>(n, D, keys, z, split_first ? 0 : -1, h->key_shared,
+                                                                   h->chain_offset);
   BJX_CHECK_LAUNCH("k_dense_normal");
   if (dense_m) return gemm(h, w, n, z, PL_P, MAT_MSQRT, p_out, nullptr, 1.f, nullptr, 0.f);  // p = L^-T z
   const bool per_chain = (h->metric_kind == BJX_METRIC_DIAG_PER_CHAIN);
@@ -568,6 +572,19 @@ int bjx_dense_velocity(bjx_handle_t h, const float* p, float* v) {
   DenseWs w;
   int rc = dense_ws(h, w);
   return rc ? rc : dense_velocity(h, w, h->cfg.n_chains, p, v);
+}
+
+// The elliptical slice prior's L z for every chain (bjx_ess.cu): z = normal(split(key_c, 4)[1], (D,)) and one
+// float32-accurate product against the planes of L = chol(cov); *lz points at the result [C, D] in the workspace.
+int bjx_dense_prior_product(bjx_handle_t h, const uint32_t* keys, const float** lz) {
+  DenseWs w;
+  int rc = dense_ws(h, w);
+  if (rc) return rc;
+  const int C = h->cfg.n_chains, D = h->cfg.dim;
+  k_dense_normal<<<g4((long long)C * D / 4), 256, 0, h->stream>>>(C, D, keys, w.v, 1, h->key_shared, h->chain_offset);
+  BJX_CHECK_LAUNCH("k_dense_normal");
+  *lz = w.p;
+  return gemm(h, w, C, w.v, PL_P, MAT_PRIOR, w.p, nullptr, 1.f, nullptr, 0.f);
 }
 
 int bjx_dense_init_state(bjx_handle_t h, const float* q, float* logp_out, float* grad_out) {

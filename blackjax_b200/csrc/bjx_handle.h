@@ -39,9 +39,9 @@ struct bjx_handle_s {
   size_t dense_bytes = 0;
   void* gemm_ws = nullptr;
   size_t gemm_ws_bytes = 0;
-  uint16_t* dense_mat_s[3] = {};       // fp16-split copies of M^-1, L^-T, target precision ([D, 3D] each)
-  const float* dense_mat_src[3] = {};  // the float32 matrices they were built from
-  unsigned dense_mat_ver[3] = {};
+  uint16_t* dense_mat_s[4] = {};       // fp16-split copies of M^-1, L^-T, target precision, prior chol(cov) ([D, 3D] each)
+  const float* dense_mat_src[4] = {};  // the float32 matrices they were built from
+  unsigned dense_mat_ver[4] = {};
   unsigned dense_version = 1;    // bumped by bjx_set_metric / bjx_set_target (contents may change behind the same pointer)
   size_t dense_bytes_built = 0;
   float* lr_block = nullptr;     // low-rank metric (owned): U [D,k] | sigma [D] | 1/sigma [D] | lambda-1 [k] | 1/sqrt(lambda)-1 [k]
@@ -62,6 +62,13 @@ struct bjx_handle_s {
   size_t sample_keys_cap = 0;
   float* gist_ws = nullptr;            // GIST scratch (bjx_gist.cu): 4 rows [C,D] and the chain queue
   size_t gist_ws_cap = 0;
+  // elliptical slice prior (bjx_ess.cu), apart from the metric: kind -1 until set; mean [D] | sqrt(cov) [D] or
+  // chol(cov) [D, D]
+  int ess_kind = -1;
+  float* ess_prior = nullptr;
+  size_t ess_prior_cap = 0;
+  float* ess_ws = nullptr;             // nu [C, D] of the big rows and the chain queue
+  size_t ess_ws_cap = 0;
   std::string err;
 };
 

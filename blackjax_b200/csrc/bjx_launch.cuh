@@ -12,7 +12,7 @@ namespace bjx {
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
 enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
                K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN, K_GIST, K_GIST_CHAINS, K_LANGEVIN,
-               K_LANGEVIN_CHAINS };
+               K_LANGEVIN_CHAINS, K_ESS, K_ESS_CHAINS };
 
 struct LaunchArgs {
   Params P;
@@ -27,6 +27,7 @@ struct LaunchArgs {
   LapsArgs laps;
   GistArgs gist;
   LangevinArgs langevin;
+  EssArgs ess;         // K_ESS / K_ESS_CHAINS: q_in, logp_in (logL), q_out, logp_out
   int grid_override;   // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
@@ -95,6 +96,27 @@ static int launch_langevin(int kernel_id, const LaunchArgs& a, dim3 grid, size_t
   else
     k_langevin_chains<R, TK, DM, KIND><<<grid, kThreads, smem, a.stream>>>(a.P, a.q_out, a.logp_out, a.g_out, a.langevin);
   return 0;
+}
+
+template <class R, int TK, bool DM, int PRIOR>
+static int launch_ess(int kernel_id, const LaunchArgs& a, dim3 grid) {
+  const size_t smem = ess_smem_bytes<TK, DM>(a.P.D);
+  if (kernel_id == K_ESS) {
+    auto kern = k_ess_transition<R, TK, DM, PRIOR>;
+    allow_dynamic_smem(kern, smem);
+    kern<<<grid, kThreads, smem, a.stream>>>(a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.ess);
+    return 0;
+  }
+  if constexpr (PRIOR != ESS_PRIOR_NU) {  // persistent grid, as K_GIST_CHAINS
+    auto kern = k_ess_chains<R, TK, DM, PRIOR>;
+    allow_dynamic_smem(kern, smem);
+    int nb = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kThreads, smem) != cudaSuccess || nb < 1) nb = 1;
+    const long long ctas = std::min<long long>(grid.x, (long long)a.grid_override * nb);
+    kern<<<dim3((unsigned)ctas), kThreads, smem, a.stream>>>(a.P, a.q_out, a.logp_out, a.ess);
+    return 0;
+  }
+  return -2;
 }
 
 template <class R, int TK, bool DM, bool GEN>
@@ -185,6 +207,19 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
         return launch_langevin<R, TK, DM, LANGEVIN_BARKER>(kernel_id, a, grid, smem);
       } else if constexpr (!GEN && R::NS <= 4) {
         if (a.langevin.kind == LANGEVIN_BARKER) return launch_langevin<R, TK, DM, LANGEVIN_BARKER>(kernel_id, a, grid, smem);
+      }
+      break;
+    case K_ESS:
+    case K_ESS_CHAINS:
+      // velocity Verlet instances only (nothing is integrated); dm selects the small dense prior (dim <= 128), the
+      // tensor-core route's nu from HBM exists for the vector rows beyond 128 dims and its loop is a launch per step
+      if constexpr (!GEN && !DM) {
+        if (a.ess.prior == ESS_PRIOR_DIAG) return launch_ess<R, TK, DM, ESS_PRIOR_DIAG>(kernel_id, a, grid);
+        if constexpr (R::VEC && R::NS >= 8) {
+          if (a.ess.prior == ESS_PRIOR_NU) return launch_ess<R, TK, DM, ESS_PRIOR_NU>(kernel_id, a, grid);
+        }
+      } else if constexpr (!GEN && R::NS <= 4) {
+        if (a.ess.prior == ESS_PRIOR_DENSE) return launch_ess<R, TK, DM, ESS_PRIOR_DENSE>(kernel_id, a, grid);
       }
       break;
     case K_NUTS_CHAINS: {

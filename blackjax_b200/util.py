@@ -246,6 +246,31 @@ def sample_barker_native(rng_key, state, logdensity_fn, step_size, num_steps, in
     return BarkerState(*final), hist, acc
 
 
+def sample_elliptical_slice_native(rng_key, state, loglikelihood_fn, mean, cov, num_steps, *, max_subiter=1000, thin=1,
+                                   keep_history=True, chain_offset=0):
+    """``run_inference_algorithm`` for elliptical slice sampling without a Python-level loop (libbjx
+    ``bjx_elliptical_slice_sample``): the same draws as ``num_steps`` calls of ``elliptical_slice`` with the step keys
+    ``split(rng_key, T)[t]``.  Returns (final EllipSliceState, positions [num_steps // thin, C, D] or None, subiter
+    int32 [num_steps, C])."""
+    from ._engine import get_engine
+    from ._lib import check, lib, ptr
+    from .mcmc.elliptical_slice import EllipSliceState, _check_cov
+    _check_cov(cov)
+    q, logl = (t.clone() for t in state)
+    eng = get_engine(q, loglikelihood_fn)
+    eng.ensure_elliptical_prior(mean, cov)
+    key = rng_key.to(q.device).contiguous()
+    if key.ndim != 1:
+        raise ValueError("sample_elliptical_slice_native takes ONE rng_key of shape [2]")
+    eng._key_mode(key, chain_offset)
+    C, D = q.shape
+    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
+    subiter = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    check(lib().bjx_elliptical_slice_sample(eng.h, ptr(key), ptr(q), ptr(logl), int(num_steps), int(max_subiter),
+                                            ptr(hist), int(thin), ptr(subiter)), eng.h)
+    return EllipSliceState(q, logl), hist, subiter
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

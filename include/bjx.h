@@ -478,6 +478,47 @@ int bjx_barker_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* 
                       const float* step_size_dev, int32_t num_steps, float* history, int32_t thin,
                       float* acceptance_history);
 
+/* ---- Elliptical slice sampling (blackjax/mcmc/elliptical_slice.py) -------------------------------------------------------
+ * State (q [C,D], logl [C]) where logl is the log-LIKELIHOOD of the handle's target; initialise it with bjx_init_state
+ * (and discard the gradient row it also writes).  The Gaussian prior N(mean, cov) is set apart from the metric, and does
+ * not change the route of any other call.  One transition of one chain, all in float32:
+ *   (key_slice, key_momentum, key_uniform, key_theta) = split(key, 4); nu = mean + S normal(key_momentum, (D,)) with
+ *   S = sqrt(cov) or chol(cov); logy = logl + log(uniform(key_uniform)); theta = 6.2831855f * uniform(key_theta), bracket
+ *   [theta - 6.2831855f, theta]; p = (q - mean) cos theta + (nu - mean) sin theta + mean; subiter = 1; while
+ *   logL(p) <= logy: theta = max(theta_min, f (theta_max - theta_min) + theta_min), f = uniform(fold_in(key_slice,
+ *   subiter)), new p, shrink the bracket towards 0, subiter += 1.  A NaN log-likelihood ends the loop and is accepted.
+ * The one deviation from the reference is the cap max_subiter (1000 in the Python API): a chain whose proposal is still
+ * below the slice after max_subiter evaluations keeps (q, logl) and reports exhausted = 1, subiter = max_subiter,
+ * theta = 0 and momentum = nu.  The reference would loop without end there (e.g. a start at logl = -inf); for a
+ * continuous likelihood and a finite start the bracket reaches float32 resolution long before 1000 sub-iterations, so
+ * the results are the reference's whenever the cap is not reached.
+ * Routes (chosen from the handle):
+ *   - every row target and row plug-in, 1 <= dim <= 1024, with a diagonal prior or a dense prior at dim <= 128;
+ *   - a dense prior at 128 < dim <= 1024 (dim % 4 == 0): chol(cov) z is a float32-accurate tensor-core product (within
+ *     about 1e-5 of the row maximum);
+ *   - every big-row target and big plug-in, 1024 < dim <= 18432 (dim % 4 == 0), with a diagonal prior.
+ * BJX_E_UNSUPPORTED: a dense prior beyond 1024 dims or at 128 < dim with dim % 4 != 0 (from bjx_set_elliptical_prior),
+ * a dense Gaussian target beyond 128 dims (the tensor-core target path), a plug-in built without the kernels of the row
+ * size, and a step or sample call before bjx_set_elliptical_prior. */
+/* kind: BJX_METRIC_DIAG (cov = variances [D]) or BJX_METRIC_DENSE (cov [D, D], chol formed in float64 on the host;
+ * BJX_E_INVALID when it is not positive definite).  mean [D].  Both are device arrays, copied into the handle. */
+int bjx_set_elliptical_prior(bjx_handle_t h, int32_t kind, const float* mean, const float* cov);
+typedef struct {            /* optional per-transition outputs (NULL => not written) */
+  float* momentum;          /* [C,D] (nu - mean) cos theta - (q - mean) sin theta + mean at the accepted theta */
+  float* theta;             /* [C] */
+  int32_t* subiter;         /* [C] likelihood evaluations of the transition */
+  uint8_t* exhausted;       /* [C] 1: max_subiter reached below the slice, state kept */
+} bjx_elliptical_slice_info;
+/* One transition; out may alias in (in place); max_subiter >= 1.  Keys follow bjx_set_key_mode. */
+int bjx_elliptical_slice_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logl_in,
+                              float* q_out, float* logl_out, int32_t max_subiter, const bjx_elliptical_slice_info* info);
+/* run_inference_algorithm (util.py:150-213): step keys = split(rng_key, num_steps) on the device, then num_steps
+ * transitions in place with no host synchronisation, bit-identical to num_steps step calls with those keys (shared step
+ * key mode, bjx_set_key_mode's chain_offset honoured).  history (optional) float32 [num_steps / thin, C, D];
+ * subiter_history (optional) int32 [num_steps, C]. */
+int bjx_elliptical_slice_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logl, int32_t num_steps,
+                                int32_t max_subiter, float* history, int32_t thin, int32_t* subiter_history);
+
 /* ---- Adjusted MCLMC tuning: adjusted_mclmc_find_L_and_step_size (blackjax/adaptation/adjusted_mclmc_adaptation.py:26-507)
  * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
  * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_adjusted_mclmc_step (BJX_E_UNSUPPORTED
