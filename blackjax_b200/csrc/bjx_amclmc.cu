@@ -66,8 +66,6 @@ extern "C" int bjx_adjusted_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key
     return bjx_fail(h, BJX_E_INVALID, "the dynamic step-count rules need random_generator_arg");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  int rc = split_step_keys(h, rng_key, num_steps);
-  if (rc) return rc;
   AmclmcArgs A{};
   A.L_factor = L_proposal_factor;
   A.n = num_integration_steps;
@@ -75,15 +73,11 @@ extern "C" int bjx_adjusted_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key
   A.min_steps = min_steps;
   A.scale = steps_scale;
   A.rga = random_generator_arg;
-  SharedStepKeys shared(h);
-  const size_t C = h->cfg.n_chains;
-  for (int t = 0; t < num_steps && rc == 0; ++t) {
+  const int C = h->cfg.n_chains;
+  return run_steps(h, rng_key, num_steps, history, thin, q, [&](int t, const uint32_t* key_t) {
     bjx_info info{};
-    info.acceptance_rate = acceptance_history ? acceptance_history + (size_t)t * C : nullptr;
-    info.num_integration_steps = steps_history ? steps_history + (size_t)t * C : nullptr;
-    rc = amclmc_transition(h, h->sample_keys + 2 * (size_t)t, q, logp, grad, q, logp, grad, step_size, step_size_dev, A,
-                           &info);
-    if (rc == 0) rc = copy_history(h, history, thin, t, q);
-  }
-  return rc;
+    info.acceptance_rate = step_row(acceptance_history, t, C);
+    info.num_integration_steps = step_row(steps_history, t, C);
+    return amclmc_transition(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, A, &info);
+  });
 }

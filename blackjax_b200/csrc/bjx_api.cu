@@ -155,12 +155,19 @@ extern "C" int bjx_create(const bjx_config* cfg, bjx_handle_t* out) {
   int* h_flag = nullptr;
   e = cudaMallocHost((void**)&h_flag, 64 * sizeof(int));
   if (e != cudaSuccess) return bjx_cuda_fail(nullptr, e, "cudaMallocHost");
+  int* chain_queue = nullptr;
+  e = cudaMalloc((void**)&chain_queue, sizeof(int));
+  if (e != cudaSuccess) {
+    cudaFreeHost(h_flag);
+    return bjx_cuda_fail(nullptr, e, "cudaMalloc");
+  }
   bjx_handle_t h = new bjx_handle_s();  // (defaults: bjx_handle.h)
   h->cfg = *cfg;
   if (!(h->cfg.divergence_threshold > 0.f)) h->cfg.divergence_threshold = 1000.f;
   h->stream = (cudaStream_t)cfg->stream;
   h->sc = sc;
   h->h_flag = h_flag;
+  h->chain_queue = chain_queue;
   *out = h;
   return 0;
 }
@@ -177,6 +184,7 @@ extern "C" int bjx_destroy(bjx_handle_t h) {
   if (h->lr_block) cudaFree(h->lr_block);
   if (h->gemm_ws) cudaFree(h->gemm_ws);
   if (h->sample_keys) cudaFree(h->sample_keys);
+  if (h->chain_queue) cudaFree(h->chain_queue);
   if (h->gist_ws) cudaFree(h->gist_ws);
   if (h->chol) cudaFree(h->chol);
   if (h->ess_prior) cudaFree(h->ess_prior);
@@ -411,6 +419,8 @@ int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, LaunchArgs& a
   const bool dm = ess ? a.ess.prior == ESS_PRIOR_DENSE
                       : (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK) &&
                             !(langevin && a.langevin.kind == LANGEVIN_MALA);  // MALA has no metric
+  if (kernel_id == K_NUTS_CHAINS || kernel_id == K_GIST_CHAINS || kernel_id == K_ESS_CHAINS)  // the persistent grids
+    BJX_CUDA(cudaMemsetAsync(h->chain_queue, 0, sizeof(int), h->stream));
   int rc;
   const int tk = target_dependent ? h->cfg.target.kind : (int)BJX_TARGET_FUNNEL;
   switch (tk) {
@@ -680,15 +690,6 @@ int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps) {
   return 0;
 }
 
-// history (optional) receives the positions after every `thin`-th transition: row (t + 1) / thin - 1 after transition t
-int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q) {
-  if (!history || ((t + 1) % thin) != 0) return 0;
-  const size_t row = (size_t)h->cfg.n_chains * h->cfg.dim;
-  BJX_CUDA(cudaMemcpyAsync(history + (size_t)((t + 1) / thin - 1) * row, q, row * sizeof(float), cudaMemcpyDeviceToDevice,
-                           h->stream));
-  return 0;
-}
-
 // run_inference_algorithm (blackjax/util.py:150-213) for HMC / multinomial HMC, natively: keys = split(rng_key,
 // num_steps) (util.py:203) on the device, then num_steps transitions enqueued back to back with NO host
 // synchronisation; per-chain keys come from the step key inside the kernel (bjx_set_key_mode's chain_offset is
@@ -699,18 +700,12 @@ extern "C" int bjx_hmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* q,
   if (!h || !rng_key || num_steps < 0 || thin < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  int rc = split_step_keys(h, rng_key, num_steps);
-  if (rc) return rc;
-  SharedStepKeys shared(h);
-  for (int t = 0; t < num_steps && rc == 0; ++t) {
+  return run_steps(h, rng_key, num_steps, history, thin, q, [&](int t, const uint32_t* key_t) {
     bjx_info info{};
-    info.acceptance_rate = acceptance_history ? acceptance_history + (size_t)t * h->cfg.n_chains : nullptr;
-    const uint32_t* key_t = h->sample_keys + 2 * (size_t)t;
-    rc = multinomial ? bjx_mhmc_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, L, &info)
-                     : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, L, &info);
-    if (rc == 0) rc = copy_history(h, history, thin, t, q);
-  }
-  return rc;
+    info.acceptance_rate = step_row(acceptance_history, t, h->cfg.n_chains);
+    return multinomial ? bjx_mhmc_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, L, &info)
+                       : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, L, &info);
+  });
 }
 
 // ---- NUTS ------------------------------------------------------------------------------------------------
@@ -892,17 +887,22 @@ extern "C" int bjx_nuts_sample(bjx_handle_t h, const uint32_t* rng_key, float* q
   if (!h || !rng_key || num_steps < 0 || thin < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  int rc = split_step_keys(h, rng_key, num_steps);
-  if (rc) return rc;
-  SharedStepKeys shared(h);
-  const size_t C = h->cfg.n_chains;
-  // Enough transitions to amortise the ragged end: the chains run decoupled, every warp taking whole chains through all
-  // num_steps transitions (k_nuts_chains).  BJX_NUTS_DECOUPLED=0 keeps the step-synchronous loop (same results).
-  static const bool decoupled_ok = [] { const char* e = getenv("BJX_NUTS_DECOUPLED"); return !(e && e[0] == '0'); }();
+  const int C = h->cfg.n_chains;
   const Route route = transition_route(h);
-  if (decoupled_ok && num_steps >= 4 && max_num_doublings > 0 && route != ROUTE_DENSE) {  // (the dense path is lock step)
+  // Too few transitions to amortise the ragged end of the decoupled chains, no tree, or the lock-step dense path: one
+  // bjx_nuts_step per transition
+  if (num_steps < 4 || max_num_doublings <= 0 || route == ROUTE_DENSE)
+    return run_steps(h, rng_key, num_steps, history, thin, q, [&](int t, const uint32_t* key_t) {
+      bjx_info info{};
+      info.acceptance_rate = step_row(acceptance_history, t, C);
+      info.num_integration_steps = step_row(num_integration_steps_history, t, C);
+      return bjx_nuts_step(h, key_t, q, logp, grad, q, logp, grad, step_size, step_size_dev, max_num_doublings, &info,
+                           nullptr, nullptr);
+    });
+  // the chains run decoupled, every warp taking whole chains through all num_steps transitions (k_nuts_chains)
+  return run_loop(h, rng_key, num_steps, history, thin, [&](const RunLoop& loop) {
     const void* ptrs[] = {q, grad};
-    rc = check_ready(h, true, ptrs, 2);
+    int rc = check_ready(h, true, ptrs, 2);
     if (rc) return rc;
     if (!logp) return bjx_fail(h, BJX_E_INVALID, "null array argument");
     rc = nuts_prepare(h, route, max_num_doublings);
@@ -911,31 +911,17 @@ extern "C" int bjx_nuts_sample(bjx_handle_t h, const uint32_t* rng_key, float* q
     a.P = make_params(h, step_size, step_size_dev);
     a.ws = h->ws;
     a.q_out = q; a.logp_out = logp; a.g_out = grad;
-    a.sample.step_keys = h->sample_keys;
-    a.sample.num_steps = num_steps;
+    a.sample.loop = loop;
     a.sample.max_doublings = max_num_doublings;
     a.sample.ckpt_smem = ckpt_in_smem(h, max_num_doublings);
-    a.sample.history = history;
-    a.sample.thin = thin;
     a.sample.acceptance_history = acceptance_history;
     a.sample.nint_history = num_integration_steps_history;
     a.sample.leapfrogs = nullptr;
-    a.sample.queue = h->ws.counters + 62;
-    a.grid_override = sm_count();  // the launcher multiplies by the CTAs that stay resident per SM
     rc = dispatch(h, K_NUTS_CHAINS, true, a);
     h->last_leaf_launches = 1;
     h->last_depth = -1;
     return rc;
-  }
-  for (int t = 0; t < num_steps && rc == 0; ++t) {
-    bjx_info info{};
-    info.acceptance_rate = acceptance_history ? acceptance_history + (size_t)t * C : nullptr;
-    info.num_integration_steps = num_integration_steps_history ? num_integration_steps_history + (size_t)t * C : nullptr;
-    rc = bjx_nuts_step(h, h->sample_keys + 2 * (size_t)t, q, logp, grad, q, logp, grad, step_size, step_size_dev,
-                       max_num_doublings, &info, nullptr, nullptr);
-    if (rc == 0) rc = copy_history(h, history, thin, t, q);
-  }
-  return rc;
+  });
 }
 
 static __global__ void k_accum_steps(int C, const int* __restrict__ n, unsigned long long* __restrict__ out) {
@@ -959,24 +945,21 @@ static int warmup_run(bjx_handle_t h, const uint32_t* rng_key, int32_t num_steps
     return bjx_fail(h, BJX_E_INVALID, "give max_num_doublings (NUTS) or num_integration_steps (HMC)");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  int rc = split_step_keys(h, rng_key, num_steps);
-  if (rc) return rc;
-  SharedStepKeys shared(h);
-  for (int t = 0; t < num_steps && rc == 0; ++t) {
+  return run_steps(h, rng_key, num_steps, nullptr, 1, q, [&](int t, const uint32_t* key_t) {
     bjx_info info{};
     info.acceptance_rate = acceptance_scratch;
     info.num_integration_steps = (leapfrog_counter && steps_scratch) ? steps_scratch : nullptr;
-    const uint32_t* key_t = h->sample_keys + 2 * (size_t)t;
-    rc = max_num_doublings > 0
-             ? bjx_nuts_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, max_num_doublings, &info, nullptr, nullptr)
-             : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, num_integration_steps, &info);
-    if (rc == 0 && info.num_integration_steps) {  // executed leapfrogs, accumulated on the device (bench.py)
+    int rc = max_num_doublings > 0
+                 ? bjx_nuts_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, max_num_doublings, &info,
+                                 nullptr, nullptr)
+                 : bjx_hmc_step(h, key_t, q, logp, grad, q, logp, grad, 0.f, step_size_chain, num_integration_steps, &info);
+    if (rc) return rc;
+    if (info.num_integration_steps) {  // executed leapfrogs, accumulated on the device (bench.py)
       k_accum_steps<<<sm_count(), 256, 0, h->stream>>>(h->cfg.n_chains, steps_scratch, leapfrog_counter);
       BJX_CHECK_LAUNCH("k_accum_steps");
     }
-    if (rc == 0) rc = update(t);
-  }
-  return rc;
+    return update(t);
+  });
 }
 
 // window_adaptation(...).run for the shared (one step size, one diagonal metric) recipe: schedule[t] = stage |

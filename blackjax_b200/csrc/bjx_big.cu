@@ -370,7 +370,7 @@ int bjx_big_hmc_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
   a.q_out = q_out; a.logp_out = logp_out; a.g_out = g_out; a.n = L; a.info = info;
   return big_dispatch(h, BK_HMC, a);
 }
-// MALA / Barker on the big rows: one transition (A.step_keys == nullptr) or the native loop (bjx_langevin.cu)
+// MALA / Barker on the big rows: one transition (A.loop.step_keys == nullptr) or the native loop (bjx_langevin.cu)
 int bjx_big_langevin(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, const float* g_in,
                      float* q_out, float* logp_out, float* g_out, float eps, const float* eps_dev, const LangevinArgs& A) {
   BigLaunchArgs a{};
@@ -380,7 +380,7 @@ int bjx_big_langevin(bjx_handle_t h, const uint32_t* keys, const float* q_in, co
   a.langevin = A;
   return big_dispatch(h, BK_LANGEVIN, a);
 }
-// Elliptical slice sampling on the big rows: one transition (A.step_keys == nullptr) or the native loop (bjx_ess.cu)
+// Elliptical slice sampling on the big rows: one transition (A.loop.step_keys == nullptr) or the native loop (bjx_ess.cu)
 int bjx_big_ess(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logl_in, float* q_out,
                 float* logl_out, const EssArgs& A) {
   BigLaunchArgs a{};

@@ -358,8 +358,8 @@ __global__ void __launch_bounds__(kBigThreads) k_big_hmc(BigParams P, const uint
 // MALA / Barker transitions (the warp kernels' langevin_transition_row, bjx_kernels.cuh) with a diagonal metric.  The
 // position and the proposal's (y, grad y), which the target addresses freely, sit in shared memory; the gradient at the
 // position is read from its [C, D] array where thread t uses elements t + 768 k (three rows fill the shared memory at
-// 18432 dims, and a fourth in registers spills).  One launch runs one transition (A.step_keys == nullptr: keys and
-// A.info as bjx_hmc_step's) or the A.num_steps transitions of the native loop, in place, with the position on chip
+// 18432 dims, and a fourth in registers spills).  One launch runs one transition (A.loop.step_keys == nullptr: keys and
+// A.info as bjx_hmc_step's) or the A.loop.num_steps transitions of the native loop, in place, with the position on chip
 // throughout and the gradient row rewritten on acceptance.
 template <int TK, int KIND>
 __global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const uint32_t* __restrict__ keys,
@@ -375,8 +375,8 @@ __global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const
   const float eps = sc.eps;
   const float* ms = P.msqrt + (size_t)c * P.imm_stride;
   const float* imm = P.imm + (size_t)c * P.imm_stride;
-  const bool loop = A.step_keys != nullptr;
-  const int T = loop ? A.num_steps : 1;
+  const bool loop = A.loop.step_keys != nullptr;
+  const int T = loop ? A.loop.num_steps : 1;
   const float* gx = g_in + ro;  // the native loop: g_in == g_out, updated on acceptance
   big_load(xs, q_in + ro, D);
   float logp_x = logp_in[c];
@@ -385,7 +385,7 @@ __global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const
   for (int t = 0; t < T; ++t) {
     // the transition's key, derived where each use needs it so that no key stays live across the target's evaluation
     auto rng = [&]() {
-      const uint32_t* kt = loop ? A.step_keys + 2 * t : keys;
+      const uint32_t* kt = loop ? A.loop.step_keys + 2 * t : keys;
       return P.key_shared ? fold_in(Key{kt[0], kt[1]}, P.chain_offset + (uint32_t)c) : Key{kt[2 * c], kt[2 * c + 1]};
     };
     float la, logp_y;  // log_p_accept; the proposal's log-density (the same in every thread)
@@ -457,8 +457,7 @@ __global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const
       logp_x = logp_y;
     }
     __syncthreads();
-    if (loop && A.history && ((t + 1) % A.thin) == 0)
-      big_store(A.history + ((size_t)((t + 1) / A.thin - 1) * P.C + c) * D, xs, D);
+    if (loop && BJX_KEEPS_HISTORY(A.loop, t)) big_store(BJX_HISTORY_ROW(A.loop, t, P.C, c, D), xs, D);
   }
   if (acc || loop) {
     big_store(q_out + ro, xs, D);
@@ -475,8 +474,9 @@ __global__ void __launch_bounds__(kBigThreads) k_big_langevin(BigParams P, const
 // Elliptical slice transitions (the warp kernels' ess_transition_row, bjx_kernels.cuh) with a diagonal prior.  The
 // proposal and its gradient scratch, which the target addresses freely, sit in shared memory; x and nu are read from
 // global memory on every sub-iteration (nu from the [C, D] scratch A.nu), each thread using the elements t + 768 k that
-// it writes itself: a third row of 18432 floats does not fit beside them.  One launch runs one transition (A.step_keys ==
-// nullptr: keys and A.info as bjx_elliptical_slice_step's) or the A.num_steps transitions of the native loop in place.
+// it writes itself: a third row of 18432 floats does not fit beside them.  One launch runs one transition
+// (A.loop.step_keys == nullptr: keys and A.info as bjx_elliptical_slice_step's) or the A.loop.num_steps transitions of
+// the native loop in place.
 template <int TK>
 __global__ void __launch_bounds__(kBigThreads) k_big_ess(BigParams P, const uint32_t* __restrict__ keys, const float* q_in,
                                                          const float* logl_in, float* q_out, float* logl_out, EssArgs A) {
@@ -484,14 +484,14 @@ __global__ void __launch_bounds__(kBigThreads) k_big_ess(BigParams P, const uint
   float *p = sm, *g = sm + P.D, *red = sm + 2 * (size_t)P.D;
   const int c = blockIdx.x, D = P.D, tid = threadIdx.x;
   const size_t ro = (size_t)c * D;
-  const bool loop = A.step_keys != nullptr;
-  const int T = loop ? A.num_steps : 1;
+  const bool loop = A.loop.step_keys != nullptr;
+  const int T = loop ? A.loop.num_steps : 1;
   const float* x = q_in + ro;  // the native loop: q_in == q_out, rewritten on acceptance
   float* nu = A.nu + ro;
   float logl_x = logl_in[c];
   for (int t = 0; t < T; ++t) {
     auto rng = [&]() {
-      const uint32_t* kt = loop ? A.step_keys + 2 * t : keys;
+      const uint32_t* kt = loop ? A.loop.step_keys + 2 * t : keys;
       return P.key_shared ? fold_in(Key{kt[0], kt[1]}, P.chain_offset + (uint32_t)c) : Key{kt[2 * c], kt[2 * c + 1]};
     };
     {
@@ -541,8 +541,8 @@ __global__ void __launch_bounds__(kBigThreads) k_big_ess(BigParams P, const uint
     } else if (q_out != q_in) {  // an out-of-place call carries the old state over
       for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = x[i];
     }
-    if (loop && A.history && ((t + 1) % A.thin) == 0) {
-      float* hrow = A.history + ((size_t)((t + 1) / A.thin - 1) * P.C + c) * D;
+    if (loop && BJX_KEEPS_HISTORY(A.loop, t)) {
+      float* hrow = BJX_HISTORY_ROW(A.loop, t, P.C, c, D);
       for (int i = tid; i < D; i += kBigThreads) hrow[i] = x[i];
     }
   }

@@ -79,10 +79,10 @@ static int ess_route(bjx_handle_t h, int& prior, bool& big) {
   return 0;
 }
 
-// The arguments every launch shares, with the handle's scratch: nu [C, D] on the big rows, then the chain queue
+// The arguments every launch shares, with the handle's scratch: nu [C, D] on the big rows
 static int ess_args(bjx_handle_t h, int prior, bool big, int max_subiter, EssArgs& A) {
   const size_t rows = big ? (size_t)h->cfg.n_chains * h->cfg.dim : 0;
-  int rc = bjx_grow(h, h->ess_ws, h->ess_ws_cap, rows + 4, sizeof(float));
+  int rc = bjx_grow(h, h->ess_ws, h->ess_ws_cap, rows, sizeof(float));
   if (rc) return rc;
   A = EssArgs{};
   A.prior = prior;
@@ -90,7 +90,6 @@ static int ess_args(bjx_handle_t h, int prior, bool big, int max_subiter, EssArg
   A.scale = h->ess_prior + h->cfg.dim;
   A.nu = big ? h->ess_ws : nullptr;
   A.max_subiter = max_subiter;
-  A.queue = reinterpret_cast<int*>(h->ess_ws + rows);
   return 0;
 }
 
@@ -143,31 +142,24 @@ extern "C" int bjx_elliptical_slice_sample(bjx_handle_t h, const uint32_t* rng_k
   bool big = false;
   if ((rc = ess_route(h, prior, big))) return rc;
   if (num_steps == 0) return 0;
-  if ((rc = split_step_keys(h, rng_key, num_steps))) return rc;
-  SharedStepKeys shared(h);
-  if (prior == ESS_PRIOR_NU) {  // per transition: the normal draw, the product and the slice kernel, all enqueued
-    for (int t = 0; t < num_steps && rc == 0; ++t) {
+  if (prior == ESS_PRIOR_NU)  // per transition: the normal draw, the product and the slice kernel, all enqueued
+    return run_steps(h, rng_key, num_steps, history, thin, q, [&](int t, const uint32_t* key_t) {
       bjx_elliptical_slice_info info{};
-      info.subiter = subiter_history ? subiter_history + (size_t)t * h->cfg.n_chains : nullptr;
-      rc = bjx_elliptical_slice_step(h, h->sample_keys + 2 * (size_t)t, q, logl, q, logl, max_subiter, &info);
-      if (rc == 0) rc = copy_history(h, history, thin, t, q);
-    }
-    return rc;
-  }
-  EssArgs A;
-  if ((rc = ess_args(h, prior, big, max_subiter, A))) return rc;
-  A.step_keys = h->sample_keys;
-  A.num_steps = num_steps;
-  A.history = history;
-  A.thin = thin;
-  A.subiter_history = subiter_history;
-  if (big) return bjx_big_ess(h, nullptr, q, logl, q, logl, A);
-  BJX_CUDA(cudaMemsetAsync(A.queue, 0, sizeof(int), h->stream));
-  LaunchArgs a{};
-  a.P = make_params(h, 0.f, nullptr);
-  a.q_out = q;
-  a.logp_out = logl;
-  a.ess = A;
-  a.grid_override = sm_count();  // the launcher multiplies by the CTAs that stay resident per SM
-  return dispatch(h, K_ESS_CHAINS, true, a);
+      info.subiter = step_row(subiter_history, t, h->cfg.n_chains);
+      return bjx_elliptical_slice_step(h, key_t, q, logl, q, logl, max_subiter, &info);
+    });
+  return run_loop(h, rng_key, num_steps, history, thin, [&](const RunLoop& loop) {
+    EssArgs A;
+    int rc = ess_args(h, prior, big, max_subiter, A);
+    if (rc) return rc;
+    A.loop = loop;
+    A.subiter_history = subiter_history;
+    if (big) return bjx_big_ess(h, nullptr, q, logl, q, logl, A);
+    LaunchArgs a{};
+    a.P = make_params(h, 0.f, nullptr);
+    a.q_out = q;
+    a.logp_out = logl;
+    a.ess = A;
+    return dispatch(h, K_ESS_CHAINS, true, a);
+  });
 }

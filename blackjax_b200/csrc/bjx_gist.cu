@@ -35,10 +35,10 @@ static int gist_supported(bjx_handle_t h, const bjx_gist_params* prm) {
   return 0;
 }
 
-// The launch arguments shared by both entry points, with the handle's scratch (4 rows [C,D] and one int: the queue)
+// The launch arguments shared by both entry points, with the handle's scratch (4 rows [C,D])
 static int gist_args(bjx_handle_t h, const bjx_gist_params* prm, float step_size, const float* step_size_dev, LaunchArgs& a) {
   const size_t rows = (size_t)4 * h->cfg.n_chains * h->cfg.dim;
-  int rc = bjx_grow(h, h->gist_ws, h->gist_ws_cap, rows + 4, sizeof(float));
+  int rc = bjx_grow(h, h->gist_ws, h->gist_ws_cap, rows, sizeof(float));
   if (rc) return rc;
   a.P = make_params(h, step_size, step_size_dev);
   a.gist.instance = prm->instance;
@@ -48,7 +48,6 @@ static int gist_args(bjx_handle_t h, const bjx_gist_params* prm, float step_size
   a.gist.max_search_steps = prm->max_search_steps;
   a.gist.asymmetric = prm->criterion == BJX_GIST_ASYMMETRIC;
   a.gist.ws = h->gist_ws;
-  a.gist.queue = reinterpret_cast<int*>(h->gist_ws + rows);
   return 0;
 }
 
@@ -98,20 +97,16 @@ extern "C" int bjx_gist_sample(bjx_handle_t h, const bjx_gist_params* params, co
   if (!rng_key || !logp || num_steps < 0 || thin < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   if ((rc = gist_supported(h, params))) return rc;
   if (num_steps == 0) return 0;
-  if ((rc = split_step_keys(h, rng_key, num_steps))) return rc;
-  SharedStepKeys shared(h);
-  LaunchArgs a{};
-  if ((rc = gist_args(h, params, step_size, step_size_dev, a))) return rc;
-  a.q_out = q;
-  a.logp_out = logp;
-  a.g_out = grad;
-  a.gist.step_keys = h->sample_keys;
-  a.gist.num_steps = num_steps;
-  a.gist.history = history;
-  a.gist.thin = thin;
-  a.gist.acceptance_history = acceptance_history;
-  a.gist.nint_history = num_integration_steps_history;
-  BJX_CUDA(cudaMemsetAsync(a.gist.queue, 0, sizeof(int), h->stream));
-  a.grid_override = sm_count();  // the launcher multiplies by the CTAs that stay resident per SM
-  return dispatch(h, K_GIST_CHAINS, true, a);
+  return run_loop(h, rng_key, num_steps, history, thin, [&](const RunLoop& loop) {
+    LaunchArgs a{};
+    int rc = gist_args(h, params, step_size, step_size_dev, a);
+    if (rc) return rc;
+    a.q_out = q;
+    a.logp_out = logp;
+    a.g_out = grad;
+    a.gist.loop = loop;
+    a.gist.acceptance_history = acceptance_history;
+    a.gist.nint_history = num_integration_steps_history;
+    return dispatch(h, K_GIST_CHAINS, true, a);
+  });
 }

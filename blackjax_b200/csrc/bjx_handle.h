@@ -60,14 +60,15 @@ struct bjx_handle_s {
   uint32_t chain_offset = 0;
   uint32_t* sample_keys = nullptr;     // [num_steps, 2] step keys of the run loops (bjx_hmc_sample, ...)
   size_t sample_keys_cap = 0;
-  float* gist_ws = nullptr;            // GIST scratch (bjx_gist.cu): 4 rows [C,D] and the chain queue
+  int* chain_queue = nullptr;          // the persistent run loops' chain queue (RunLoop::queue), one int
+  float* gist_ws = nullptr;            // GIST scratch (bjx_gist.cu): 4 rows [C,D]
   size_t gist_ws_cap = 0;
   // elliptical slice prior (bjx_ess.cu), apart from the metric: kind -1 until set; mean [D] | sqrt(cov) [D] or
   // chol(cov) [D, D]
   int ess_kind = -1;
   float* ess_prior = nullptr;
   size_t ess_prior_cap = 0;
-  float* ess_ws = nullptr;             // nu [C, D] of the big rows and the chain queue
+  float* ess_ws = nullptr;             // nu [C, D] of the big rows
   size_t ess_ws_cap = 0;
   std::string err;
 };
@@ -130,6 +131,33 @@ inline long long history_slice_chains(long long max_history_bytes, int n, int D,
     cudaError_t e_ = cudaGetLastError();                          \
     if (e_ != cudaSuccess) return bjx_cuda_fail(h, e_, where);    \
   } while (0)
+
+// A native run loop: the step keys split(rng_key, num_steps) into h->sample_keys, then run(loop) with every chain's key
+// derived from the step key (SharedStepKeys).
+template <class Run>
+int run_loop(bjx_handle_t h, const uint32_t* rng_key, int num_steps, float* history, int thin, Run run) {
+  int rc = split_step_keys(h, rng_key, num_steps);
+  if (rc) return rc;
+  SharedStepKeys shared(h);
+  return run(bjx::RunLoop{h->sample_keys, num_steps, history, thin, h->chain_queue});
+}
+
+// The run loop of one transition per step enqueued from the host: step(t, step key t) for every t, each followed by the
+// copy of the positions q into their history row; nothing waits for the device.
+template <class Step>
+int run_steps(bjx_handle_t h, const uint32_t* rng_key, int num_steps, float* history, int thin, const float* q, Step step) {
+  return run_loop(h, rng_key, num_steps, history, thin, [&](const bjx::RunLoop& loop) {
+    const size_t row = (size_t)h->cfg.n_chains * h->cfg.dim;
+    int rc = 0;
+    for (int t = 0; t < num_steps && rc == 0; ++t) {
+      rc = step(t, loop.step_keys + 2 * (size_t)t);
+      if (rc == 0 && BJX_KEEPS_HISTORY(loop, t))
+        BJX_CUDA(cudaMemcpyAsync(BJX_HISTORY_ROW(loop, t, 1, 0, row), q, row * sizeof(float), cudaMemcpyDeviceToDevice,
+                                 h->stream));
+    }
+    return rc;
+  });
+}
 
 // The tuners' ESS stage, one slice of chains [c0, c0 + n) at a time: n_steps calls of step(c0, n, t), each followed by a
 // copy of the slice's positions q into history row t; then the per-chain ESS of the slice into ess [n, D] and

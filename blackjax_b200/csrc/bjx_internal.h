@@ -74,8 +74,6 @@ int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, bjx::LaunchAr
 int check_ready(bjx_handle_t h, bool need_metric, const void* const* ptrs, int n);
 // split(rng_key, num_steps) into h->sample_keys (util.py:203)
 int split_step_keys(bjx_handle_t h, const uint32_t* rng_key, int num_steps);
-// history row (t + 1) / thin - 1 = q after transition t, when (t + 1) % thin == 0
-int copy_history(bjx_handle_t h, float* history, int thin, int t, const float* q);
 // L = chol(a) (lower, row-major [D, D]) in float64 from the float32 [D, D] a; false when a is not positive definite
 bool cholesky_f64(const std::vector<float>& a, int D, std::vector<double>& L);
 // bjx_mclmc.cu: dim >= 2, a diagonal metric and the row kernels, or BJX_E_UNSUPPORTED with "<name> ..." as the reason

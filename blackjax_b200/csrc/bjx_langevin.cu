@@ -83,24 +83,21 @@ static int langevin_sample(bjx_handle_t h, int kind, const uint32_t* rng_key, fl
   bool big = false;
   if ((rc = langevin_supported(h, kind, big))) return rc;
   if (num_steps == 0) return 0;
-  if ((rc = split_step_keys(h, rng_key, num_steps))) return rc;
-  SharedStepKeys shared(h);
-  LangevinArgs A{};
-  A.kind = kind;
-  A.chol = h->chol;
-  A.step_keys = h->sample_keys;
-  A.num_steps = num_steps;
-  A.history = history;
-  A.thin = thin;
-  A.acceptance_history = acceptance_history;
-  if (big) return bjx_big_langevin(h, nullptr, q, logp, grad, q, logp, grad, step_size, step_size_dev, A);
-  LaunchArgs a{};
-  a.P = make_params(h, step_size, step_size_dev);
-  a.q_out = q;
-  a.logp_out = logp;
-  a.g_out = grad;
-  a.langevin = A;
-  return dispatch(h, K_LANGEVIN_CHAINS, true, a);
+  return run_loop(h, rng_key, num_steps, history, thin, [&](const RunLoop& loop) {
+    LangevinArgs A{};
+    A.kind = kind;
+    A.chol = h->chol;
+    A.loop = loop;
+    A.acceptance_history = acceptance_history;
+    if (big) return bjx_big_langevin(h, nullptr, q, logp, grad, q, logp, grad, step_size, step_size_dev, A);
+    LaunchArgs a{};
+    a.P = make_params(h, step_size, step_size_dev);
+    a.q_out = q;
+    a.logp_out = logp;
+    a.g_out = grad;
+    a.langevin = A;
+    return dispatch(h, K_LANGEVIN_CHAINS, true, a);
+  });
 }
 
 extern "C" int bjx_mala_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in,

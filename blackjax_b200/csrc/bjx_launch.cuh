@@ -28,7 +28,6 @@ struct LaunchArgs {
   GistArgs gist;
   LangevinArgs langevin;
   EssArgs ess;         // K_ESS / K_ESS_CHAINS: q_in, logp_in (logL), q_out, logp_out
-  int grid_override;   // persistent launches: number of CTAs
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
   float *q_out, *logp_out, *g_out;
@@ -88,6 +87,19 @@ static void allow_dynamic_smem(K kern, size_t bytes) {
   if (bytes > 48 * 1024 - 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 }
 
+// A persistent grid over the chains (k_nuts_chains, k_gist_chains, k_ess_chains), whose warps take the chains from the
+// queue dispatch() zeroed: every CTA that stays resident (registers, shared memory) on each SM, at most one per
+// kWarpsPerBlock chains.
+template <class K, class... Args>
+static void launch_persistent(K kern, const LaunchArgs& a, size_t smem, Args... args) {
+  allow_dynamic_smem(kern, smem);
+  int nb = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kThreads, smem) != cudaSuccess || nb < 1) nb = 1;
+  const long long want = ((long long)a.P.C + kWarpsPerBlock - 1) / kWarpsPerBlock;
+  const long long ctas = std::min<long long>(want, (long long)sm_count() * nb);
+  kern<<<dim3((unsigned)ctas), kThreads, smem, a.stream>>>(args...);
+}
+
 template <class R, int TK, bool DM, int KIND>
 static int launch_langevin(int kernel_id, const LaunchArgs& a, dim3 grid, size_t smem) {
   if (kernel_id == K_LANGEVIN)
@@ -107,13 +119,8 @@ static int launch_ess(int kernel_id, const LaunchArgs& a, dim3 grid) {
     kern<<<grid, kThreads, smem, a.stream>>>(a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.ess);
     return 0;
   }
-  if constexpr (PRIOR != ESS_PRIOR_NU) {  // persistent grid, as K_GIST_CHAINS
-    auto kern = k_ess_chains<R, TK, DM, PRIOR>;
-    allow_dynamic_smem(kern, smem);
-    int nb = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kThreads, smem) != cudaSuccess || nb < 1) nb = 1;
-    const long long ctas = std::min<long long>(grid.x, (long long)a.grid_override * nb);
-    kern<<<dim3((unsigned)ctas), kThreads, smem, a.stream>>>(a.P, a.q_out, a.logp_out, a.ess);
+  if constexpr (PRIOR != ESS_PRIOR_NU) {
+    launch_persistent(k_ess_chains<R, TK, DM, PRIOR>, a, smem, a.P, a.q_out, a.logp_out, a.ess);
     return 0;
   }
   return -2;
@@ -187,17 +194,10 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
       kern<<<grid, block, gsm, st>>>(a.P, a.keys, a.q_in, a.logp_in, a.g_in, a.q_out, a.logp_out, a.g_out, a.gist);
       return 0;
     }
-    case K_GIST_CHAINS: {  // persistent grid, as K_NUTS_CHAINS
-      auto kern = k_gist_chains<R, TK, DM, GEN>;
-      int nb = 1;
-      const size_t gsm = gist_smem_bytes<R, TK, DM>(a.P.D);
-      allow_dynamic_smem(kern, gsm);
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kThreads, gsm) != cudaSuccess || nb < 1) nb = 1;
-      const long long want = ((long long)a.P.C + kWarpsPerBlock - 1) / kWarpsPerBlock;
-      const long long ctas = std::min<long long>(want, (long long)a.grid_override * nb);
-      kern<<<dim3((unsigned)ctas), block, gsm, st>>>(a.P, a.q_out, a.logp_out, a.g_out, a.gist);
+    case K_GIST_CHAINS:
+      launch_persistent(k_gist_chains<R, TK, DM, GEN>, a, gist_smem_bytes<R, TK, DM>(a.P.D), a.P, a.q_out,
+                        a.logp_out, a.g_out, a.gist);
       return 0;
-    }
     case K_LANGEVIN:
     case K_LANGEVIN_CHAINS:
       // velocity Verlet instances only (no integrator here); MALA has no metric (dispatched as diagonal), Barker's dense
@@ -222,17 +222,11 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
         if (a.ess.prior == ESS_PRIOR_DENSE) return launch_ess<R, TK, DM, ESS_PRIOR_DENSE>(kernel_id, a, grid);
       }
       break;
-    case K_NUTS_CHAINS: {
-      size_t sm_bytes = smem + (a.sample.ckpt_smem ? sizeof(float) * kWarpsPerBlock * 2 * a.sample.max_doublings * a.P.D : 0);
-      // persistent grid: every CTA that fits (registers, checkpoint shared memory) on each of the grid_override SMs
-      auto kern = k_nuts_chains<R, TK, DM, GEN>;
-      int nb = 1;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kThreads, sm_bytes) != cudaSuccess || nb < 1) nb = 1;
-      const long long want = ((long long)a.P.C + kWarpsPerBlock - 1) / kWarpsPerBlock;
-      const long long ctas = std::min<long long>(want, (long long)a.grid_override * nb);
-      kern<<<dim3((unsigned)ctas), block, sm_bytes, st>>>(a.P, a.ws, a.q_out, a.logp_out, a.g_out, a.sample);
+    case K_NUTS_CHAINS:  // the row and the checkpoints of every doubling in shared memory
+      launch_persistent(k_nuts_chains<R, TK, DM, GEN>, a,
+                        smem + (a.sample.ckpt_smem ? sizeof(float) * kWarpsPerBlock * 2 * a.sample.max_doublings * a.P.D : 0),
+                        a.P, a.ws, a.q_out, a.logp_out, a.g_out, a.sample);
       return 0;
-    }
     case K_NUTS_DOUBLING:
       if (a.n_in_dev)
         k_nuts_doubling<R, TK, DM, GEN, true><<<grid, block, smem, st>>>(a.P, a.ws, a.depth, a.depth_end, a.n, a.list_in, a.n_in,

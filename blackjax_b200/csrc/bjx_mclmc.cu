@@ -91,15 +91,9 @@ extern "C" int bjx_mclmc_sample(bjx_handle_t h, const uint32_t* rng_key, float* 
   if (!h || !rng_key || num_steps < 0 || thin < 1) return bjx_fail(h, BJX_E_INVALID, "bad argument");
   BJX_CUDA(cudaSetDevice(h->cfg.device));
   if (num_steps == 0) return 0;
-  int rc = split_step_keys(h, rng_key, num_steps);
-  if (rc) return rc;
-  SharedStepKeys shared(h);
-  for (int t = 0; t < num_steps && rc == 0; ++t) {
+  return run_steps(h, rng_key, num_steps, history, thin, q, [&](int t, const uint32_t* key_t) {
     bjx_mclmc_info info{};
-    info.energy_change = energy_change_history ? energy_change_history + (size_t)t * h->cfg.n_chains : nullptr;
-    rc = bjx_mclmc_step(h, h->sample_keys + 2 * (size_t)t, q, p, logp, grad, step_size, step_size_dev, L, L_dev,
-                        energy_cutoff, &info);
-    if (rc == 0) rc = copy_history(h, history, thin, t, q);
-  }
-  return rc;
+    info.energy_change = step_row(energy_change_history, t, h->cfg.n_chains);
+    return bjx_mclmc_step(h, key_t, q, p, logp, grad, step_size, step_size_dev, L, L_dev, energy_cutoff, &info);
+  });
 }

@@ -4,6 +4,19 @@ import torch
 from . import random as bjx_random
 
 
+def _native_run(name, rng_key, eng, q, num_steps, thin, keep_history, chain_offset, *stats):
+    """What every ``sample_*_native`` shares once the engine is set up: the one step key on the device (shared step-key
+    mode from ``chain_offset``), the history [num_steps // thin, C, D] or None, and one [num_steps, C] array per dtype in
+    ``stats``.  Returns (key, history, *stats)."""
+    key = rng_key.to(q.device).contiguous()
+    if key.ndim != 1:
+        raise ValueError(f"sample_{name}_native takes ONE rng_key of shape [2]")
+    eng._key_mode(key, chain_offset)
+    C, D = q.shape
+    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
+    return (key, hist, *(torch.empty(num_steps, C, dtype=dt, device=q.device) for dt in stats))
+
+
 def sample_hmc_native(rng_key, state, logdensity_fn, step_size, inverse_mass_matrix, num_integration_steps, num_steps,
                       *, multinomial=False, thin=1, keep_history=True, chain_offset=0):
     """``run_inference_algorithm`` for HMC / multinomial HMC without a Python-level loop: libbjx ``bjx_hmc_sample``
@@ -16,13 +29,7 @@ def sample_hmc_native(rng_key, state, logdensity_fn, step_size, inverse_mass_mat
     q, logp, g = (t.clone() for t in state)
     eng = get_engine(q, logdensity_fn)
     eng.ensure_metric(inverse_mass_matrix)
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError("sample_hmc_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    key, hist, acc = _native_run("hmc", rng_key, eng, q, num_steps, thin, keep_history, chain_offset, torch.float32)
     eps, eps_dev = eng._eps(step_size)
     check(lib().bjx_hmc_sample(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev), int(num_integration_steps),
                                int(num_steps), int(bool(multinomial)), ptr(hist), int(thin), ptr(acc)), eng.h)
@@ -40,14 +47,8 @@ def sample_nuts_native(rng_key, state, logdensity_fn, step_size, inverse_mass_ma
     q, logp, g = (t.clone() for t in state)
     eng = get_engine(q, logdensity_fn, max_tree_depth=max(10, max_num_doublings))
     eng.ensure_metric(inverse_mass_matrix)
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError("sample_nuts_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
-    n_int = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    key, hist, acc, n_int = _native_run("nuts", rng_key, eng, q, num_steps, thin, keep_history, chain_offset,
+                                        torch.float32, torch.int32)
     eps, eps_dev = eng._eps(step_size)
     check(lib().bjx_nuts_sample(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev), int(max_num_doublings),
                                 int(num_steps), ptr(hist), int(thin), ptr(acc), ptr(n_int)), eng.h)
@@ -69,18 +70,12 @@ def sample_mclmc_native(rng_key, state, logdensity_fn, L, step_size, num_steps, 
     eng = get_engine(q, logdensity_fn)
     eng.set_integrator(integrators.as_coefficients(integrator))
     eng.ensure_metric(metric_tensor(eng, inverse_mass_matrix), diagonal_only=True)
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError("sample_mclmc_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    de = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    key, hist, de = _native_run("mclmc", rng_key, eng, q, num_steps, thin, keep_history, chain_offset, torch.float32)
     eps, eps_dev = eng._eps(step_size)
     L, L_dev = eng._eps(L, "L")
     check(lib().bjx_mclmc_sample(eng.h, ptr(key), ptr(q), ptr(p), ptr(logp), ptr(g), eps, ptr(eps_dev), L, ptr(L_dev),
-                                 energy_cutoff(D, desired_energy_var_max_ratio, desired_energy_var), int(num_steps),
-                                 ptr(hist), int(thin), ptr(de)), eng.h)
+                                 energy_cutoff(q.shape[1], desired_energy_var_max_ratio, desired_energy_var),
+                                 int(num_steps), ptr(hist), int(thin), ptr(de)), eng.h)
     return IntegratorState(q, p, logp, g), hist, de
 
 
@@ -139,15 +134,10 @@ def sample_adjusted_mclmc_native(rng_key, state, logdensity_fn, step_size, num_s
     eng = get_engine(q, logdensity_fn, divergence_threshold=divergence_threshold)
     eng.set_integrator(integrators.as_coefficients(integrator))
     eng.ensure_metric(metric_tensor(eng, inverse_mass_matrix), diagonal_only=True)
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError("sample_adjusted_mclmc_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
-    steps = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    key, hist, acc, steps = _native_run("adjusted_mclmc", rng_key, eng, q, num_steps, thin, keep_history, chain_offset,
+                                        torch.float32, torch.int32)
     eps, eps_dev = eng._eps(step_size)
+    C = q.shape[0]
     if avg_dev is not None and tuple(avg_dev.shape) != (C,):
         raise ValueError(f"per-chain average trajectory lengths must have shape ({C},)")
     check(lib().bjx_set_integration_steps_avg(eng.h, ptr(avg_dev)), eng.h)
@@ -187,14 +177,8 @@ def sample_gist_native(rng_key, state, logdensity_fn, step_size, inverse_mass_ma
     eng = get_engine(q, logdensity_fn, divergence_threshold=divergence_threshold)
     eng.set_integrator(integrators.as_coefficients(integrator or integrators.velocity_verlet))
     eng.ensure_metric(inverse_mass_matrix)
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError("sample_gist_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
-    n_int = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    key, hist, acc, n_int = _native_run("gist", rng_key, eng, q, num_steps, thin, keep_history, chain_offset,
+                                        torch.float32, torch.int32)
     eps, eps_dev = eng._eps(step_size)
     check(lib().bjx_gist_sample(eng.h, tuning.params, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev),
                                 int(num_steps), ptr(hist), int(thin), ptr(acc), ptr(n_int)), eng.h)
@@ -212,13 +196,7 @@ def _sample_langevin_native(sampler, rng_key, state, logdensity_fn, step_size, n
         from .mcmc import barker
         barker.install_metric(eng, inverse_mass_matrix)
         fn = lib().bjx_barker_sample
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError(f"sample_{sampler}_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    acc = torch.empty(num_steps, C, dtype=torch.float32, device=q.device)
+    key, hist, acc = _native_run(sampler, rng_key, eng, q, num_steps, thin, keep_history, chain_offset, torch.float32)
     eps, eps_dev = eng._eps(step_size)
     check(fn(eng.h, ptr(key), ptr(q), ptr(logp), ptr(g), eps, ptr(eps_dev), int(num_steps), ptr(hist), int(thin),
              ptr(acc)), eng.h)
@@ -259,13 +237,8 @@ def sample_elliptical_slice_native(rng_key, state, loglikelihood_fn, mean, cov, 
     q, logl = (t.clone() for t in state)
     eng = get_engine(q, loglikelihood_fn)
     eng.ensure_elliptical_prior(mean, cov)
-    key = rng_key.to(q.device).contiguous()
-    if key.ndim != 1:
-        raise ValueError("sample_elliptical_slice_native takes ONE rng_key of shape [2]")
-    eng._key_mode(key, chain_offset)
-    C, D = q.shape
-    hist = torch.empty(num_steps // thin, C, D, dtype=torch.float32, device=q.device) if keep_history else None
-    subiter = torch.empty(num_steps, C, dtype=torch.int32, device=q.device)
+    key, hist, subiter = _native_run("elliptical_slice", rng_key, eng, q, num_steps, thin, keep_history, chain_offset,
+                                     torch.int32)
     check(lib().bjx_elliptical_slice_sample(eng.h, ptr(key), ptr(q), ptr(logl), int(num_steps), int(max_subiter),
                                             ptr(hist), int(thin), ptr(subiter)), eng.h)
     return EllipSliceState(q, logl), hist, subiter

@@ -1,5 +1,5 @@
-"""Decoupled-chains NUTS sampler (bjx_nuts_sample / k_nuts_chains) vs the step-synchronous loop: same draws, time per
-transition.  usage: python scripts/nuts_decoupled.py [C] [D] [T]   (BJX_NUTS_DECOUPLED=0 in the env selects the old loop)"""
+"""Decoupled-chains NUTS sampler (bjx_nuts_sample / k_nuts_chains) vs T calls of the step kernel (nuts.step with the keys
+split(rng_key, T)): same draws, time per transition.  usage: python scripts/nuts_decoupled.py [C] [D] [T]"""
 import os
 import sys
 
@@ -21,15 +21,30 @@ eps = 0.25
 # burn in so that the trees have their stationary depth profile
 st, _, _, _ = bj.sample_nuts_native(bj.random.key(1, dev), st, tgt, eps, imm, 40, keep_history=False)
 torch.cuda.synchronize()
-res = {}
+alg = bj.nuts(tgt, eps, imm, max_num_doublings=10)
+key = bj.random.key(2, dev)
+
+
+def decoupled():
+    fin, _, _, n_int = bj.sample_nuts_native(key, st, tgt, eps, imm, T, keep_history=False)
+    return fin, n_int.sum()
+
+
+def stepwise():
+    s, lf = st, 0
+    for k in bj.random.split(key, T):
+        s, info = alg.step(k, s)
+        lf = lf + info.num_integration_steps.sum()
+    return s, lf
+
+
 for rep in range(3):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fin, _, acc, n_int = bj.sample_nuts_native(bj.random.key(2, dev), st, tgt, eps, imm, T, keep_history=False)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1)
-    lf = int(n_int.sum())
-    print(f"decoupled={os.environ.get('BJX_NUTS_DECOUPLED', '1')} C={C} D={D} T={T}: {ms / T:.4f} ms/transition, "
-          f"{lf / ms * 1e3:.3e} leapfrogs/s, mean tree {lf / (C * T):.2f}, checksum {float(fin.position.double().sum()):.9e} "
-          f"{int(n_int.sum())}")
+    for name, run in (("decoupled", decoupled), ("step kernel", stepwise)):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        fin, lf = run()
+        e1.record()
+        torch.cuda.synchronize()
+        ms, lf = e0.elapsed_time(e1), int(lf)
+        print(f"{name} C={C} D={D} T={T}: {ms / T:.4f} ms/transition, {lf / ms * 1e3:.3e} leapfrogs/s, "
+              f"mean tree {lf / (C * T):.2f}, checksum {float(fin.position.double().sum()):.9e} {lf}")

@@ -83,7 +83,7 @@ def _set_metric(lib, h, metric, D, dev):
     return lib.bjx_set_metric(h, _lib.METRIC_DENSE_PER_CHAIN, dev(imm))
 
 
-def _transition_codes(lib, h, D, dev, rs):
+def _transition_codes(lib, h, D, metric, dev, rs):
     """Return code of every entry point, in a fixed order, on one handle (metric and integrator already set)."""
     Cn = N_CHAINS
     q, p, g = (dev(0.1 * rs.standard_normal((Cn, D))) for _ in range(3))
@@ -107,8 +107,36 @@ def _transition_codes(lib, h, D, dev, rs):
     codes["ghmc_step"] = lib.bjx_ghmc_step(h, keys, q, p, logp, g, slice_, eps, None, 0.5, None, 0.1, None, None, None,
                                            1, 0, 0, None)
     codes["nuts_step"] = lib.bjx_nuts_step(h, keys, q, logp, g, q, logp, g, eps, None, 2, None, None, None)
-    codes["hmc_sample"] = lib.bjx_hmc_sample(h, rng_key, q, logp, g, eps, None, 2, 4, 0, None, 1, None)
-    codes["nuts_sample"] = lib.bjx_nuts_sample(h, rng_key, q, logp, g, eps, None, 2, 4, None, 1, None, None)
+    gist = _lib.GistParams(_lib.GIST_TRAJECTORY_LENGTH, 0.5, 8, 0, 0, _lib.GIST_SYMMETRIC)
+    # every native loop, then the argument checks each runs before or after its route: num_steps = 0 and thin = 0
+    sample = {
+        "hmc_sample": lambda n, thin: lib.bjx_hmc_sample(h, rng_key, q, logp, g, eps, None, 2, n, 0, None, thin, None),
+        "nuts_sample": lambda n, thin: lib.bjx_nuts_sample(h, rng_key, q, logp, g, eps, None, 2, n, None, thin, None,
+                                                           None),
+        "mclmc_sample": lambda n, thin: lib.bjx_mclmc_sample(h, rng_key, q, p, logp, g, eps, None, 1.0, None, 0.1, n,
+                                                             None, thin, None),
+        "adjusted_mclmc_sample": lambda n, thin: lib.bjx_adjusted_mclmc_sample(
+            h, rng_key, q, logp, g, eps, None, 1.0, _lib.AMCLMC_STEPS_FIXED, 2, 1.0, 1, None, n, None, thin, None, None),
+        "gist_sample": lambda n, thin: lib.bjx_gist_sample(h, C.byref(gist), rng_key, q, logp, g, eps, None, n, None,
+                                                           thin, None, None),
+        "mala_sample": lambda n, thin: lib.bjx_mala_sample(h, rng_key, q, logp, g, eps, None, n, None, thin, None),
+        "barker_sample": lambda n, thin: lib.bjx_barker_sample(h, rng_key, q, logp, g, eps, None, n, None, thin, None),
+        "elliptical_slice_sample": lambda n, thin: lib.bjx_elliptical_slice_sample(h, rng_key, q, logp, n, 8, None,
+                                                                                   thin, None),
+    }
+    for name in ("hmc_sample", "nuts_sample", "mclmc_sample", "adjusted_mclmc_sample", "gist_sample", "mala_sample",
+                 "barker_sample"):
+        codes[name] = sample[name](4, 1)
+    # no prior yet on the handle's first integrator; the second finds the one set below
+    codes["elliptical_slice_sample_no_prior"] = sample["elliptical_slice_sample"](4, 1)
+    # a dense metric grid point takes the dense prior: the small matvec, the tensor-core product or its refusal
+    dense = metric == "dense"
+    codes["set_elliptical_prior"] = lib.bjx_set_elliptical_prior(
+        h, _lib.METRIC_DENSE if dense else _lib.METRIC_DIAG, dev(np.zeros(D)), dev(np.eye(D) if dense else np.ones(D)))
+    codes["elliptical_slice_sample"] = sample["elliptical_slice_sample"](4, 1)
+    for name, call in sample.items():
+        codes[f"{name}_num_steps_0"] = call(0, 1)
+        codes[f"{name}_thin_0"] = call(4, 0)
     codes["synchronize"] = lib.bjx_synchronize(h)
     return codes
 
@@ -132,7 +160,7 @@ def routing_codes():
                     if rc_create == 0:
                         codes["set_metric"] = rc_metric
                         codes["set_integrator"] = lib.bjx_set_integrator(h, (C.c_float * len(coef))(*coef), len(coef))
-                        codes.update(_transition_codes(lib, h, D, dev, rs))
+                        codes.update(_transition_codes(lib, h, D, metric, dev, rs))
                     out[f"{target}/{D}/{metric}/{integ}"] = codes
                 if rc_create == 0:
                     assert lib.bjx_destroy(h) == 0
