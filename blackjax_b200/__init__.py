@@ -27,8 +27,9 @@ from .mcmc import adjusted_mclmc_dynamic as _adjusted_mclmc_dynamic
 from .util import run_inference_algorithm, sample_hmc_native, sample_mclmc_native, sample_nuts_native  # noqa: F401
 from .util import sample_adjusted_mclmc_native, sample_gist_native  # noqa: F401
 from .util import sample_barker_native, sample_mala_native  # noqa: F401
-from .util import sample_elliptical_slice_native  # noqa: F401
+from .util import sample_elliptical_slice_native, sample_slice_sampling_native  # noqa: F401
 from .mcmc import elliptical_slice as _elliptical_slice
+from .mcmc import slice as _slice
 from .mcmc import barker as _barker
 from .mcmc import mala as _mala
 from .mcmc.composed import step_size as _gist_step_size
@@ -65,5 +66,6 @@ barker = GenerateSamplingAPI(_barker.as_top_level_api, _barker.init, _barker.bui
 barker_proposal = barker  # blackjax/__init__.py:141
 elliptical_slice = GenerateSamplingAPI(_elliptical_slice.as_top_level_api, _elliptical_slice.init,  # blackjax/__init__.py:134
                                        _elliptical_slice.build_kernel)
+slice_sampling = GenerateSamplingAPI(_slice.as_top_level_api, _slice.init, _slice.build_kernel)  # blackjax/__init__.py:134
 
 __version__ = "0.1.0"

@@ -391,6 +391,45 @@ class Engine:
                                               C.byref(info)), self.h)
         return qo, lo
 
+    def ensure_slice_scale(self, scale):
+        """Install slice sampling's direction scale (libbjx ``bjx_set_slice_direction_scale``) unless this exact content
+        is installed, keyed as ``ensure_elliptical_prior``: a scalar (expanded to [D]), [D] or [D, D]."""
+        if isinstance(scale, torch.Tensor):
+            key = (scale.data_ptr(), tuple(scale.shape), scale._version, str(scale.device))
+        else:
+            key = ("scalar", float(scale)) if np.ndim(scale) == 0 else None
+        given = scale
+        if key is not None and key == getattr(self, "_slice_scale_key", None):
+            return
+        s = torch.as_tensor(scale, dtype=torch.float32, device=self.device)
+        if s.ndim == 0:
+            s = s.expand(self.D)
+        if s.ndim == 1 and s.shape[0] == self.D:
+            kind = _lib.METRIC_DIAG
+        elif s.ndim == 2 and tuple(s.shape) == (self.D, self.D):
+            kind = _lib.METRIC_DENSE
+        else:
+            raise ValueError(f"scale has shape {tuple(s.shape)}, expected (), ({self.D},) or ({self.D}, {self.D})")
+        s = s.contiguous()
+        check(lib().bjx_set_slice_direction_scale(self.h, kind, ptr(s)), self.h)
+        self._slice_scale = (given, s)  # the key's tensor stays alive, so its address is not reused
+        self._slice_scale_key = key
+
+    def slice_step(self, keys, q, logp, width, interval, max_expansions, max_shrinkage, out=None, info_fields=None,
+                   chain_offset=0):
+        """One slice sampling transition (libbjx ``bjx_slice_step``) along a direction of the installed scale."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        logp = _f32(logp, (self.C,), "logdensity")
+        qo, lo = out if out is not None else (torch.empty_like(q), torch.empty_like(logp))
+        w, w_dev = self._eps(width, "width")
+        info = self._info(info_fields or {}, _lib.SliceInfo)
+        check(lib().bjx_slice_step(self.h, ptr(keys), ptr(q), ptr(logp), ptr(qo), ptr(lo), w, ptr(w_dev), int(interval),
+                                   int(max_expansions), int(max_shrinkage), C.byref(info)), self.h)
+        self._width_keepalive = w_dev  # the launch is asynchronous
+        return qo, lo
+
     def adjusted_mclmc_num_steps(self, device_rule, avg, random_generator_arg):
         """The step counts int32 [C] of a dynamic rule ``device_rule = (rule, min_steps)`` at a per-chain ``avg`` [C]
         (libbjx ``bjx_adjusted_mclmc_num_steps``); random_generator_arg [C, 2] is read, not advanced.  The fixed rule

@@ -390,3 +390,13 @@ int bjx_big_ess(bjx_handle_t h, const uint32_t* keys, const float* q_in, const f
   a.ess = A;
   return big_dispatch(h, BK_ESS, a);
 }
+// Slice sampling on the big rows: one transition (A.loop.step_keys == nullptr) or the native loop (bjx_slice.cu)
+int bjx_big_slice(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, float* q_out,
+                  float* logp_out, float width, const float* width_dev, const SliceArgs& A) {
+  BigLaunchArgs a{};
+  a.P = big_params(h, width, width_dev);
+  a.keys = keys; a.q_in = q_in; a.logp_in = logp_in;
+  a.q_out = q_out; a.logp_out = logp_out;
+  a.slice = A;
+  return big_dispatch(h, BK_SLICE, a);
+}

@@ -549,8 +549,87 @@ __global__ void __launch_bounds__(kBigThreads) k_big_ess(BigParams P, const uint
   if (tid == 0) logl_out[c] = logl_x;
 }
 
+
+// Slice sampling transitions (the warp kernels' slice_transition_row and SliceMachine, bjx_kernels.cuh) with a [D]
+// direction scale.  As in k_big_ess, the candidate x + t d and its gradient scratch sit in shared memory, x is re-read
+// from its row on every evaluation and d lives in the [C, D] scratch A.dir, each thread using the elements t + 768 k
+// that it writes itself.  One launch runs one transition (A.loop.step_keys == nullptr: keys and A.info as
+// bjx_slice_step's) or the A.loop.num_steps transitions of the native loop in place.
+template <int TK>
+__global__ void __launch_bounds__(kBigThreads) k_big_slice(BigParams P, const uint32_t* __restrict__ keys, const float* q_in,
+                                                           const float* logp_in, float* q_out, float* logp_out,
+                                                           SliceArgs A) {
+  extern __shared__ __align__(16) float sm[];
+  float *p = sm, *g = sm + P.D, *red = sm + 2 * (size_t)P.D;
+  const int c = blockIdx.x, D = P.D, tid = threadIdx.x;
+  const size_t ro = (size_t)c * D;
+  const bool loop = A.loop.step_keys != nullptr;
+  const int T = loop ? A.loop.num_steps : 1;
+  const float* x = q_in + ro;  // the native loop: q_in == q_out, rewritten on acceptance
+  float* d = A.dir + ro;
+  float logp_x = logp_in[c];
+  unsigned long long evals = 0;
+  for (int t = 0; t < T; ++t) {
+    auto rng = [&]() {
+      const uint32_t* kt = loop ? A.loop.step_keys + 2 * t : keys;
+      return P.key_shared ? fold_in(Key{kt[0], kt[1]}, P.chain_offset + (uint32_t)c) : Key{kt[2 * c], kt[2 * c + 1]};
+    };
+    {  // d = n / |n|, n = 0 + scale z
+      const Key prop_key = fold_in(rng(), 0u);
+      float sq[1] = {0.f};
+      for (int i = tid; i < D; i += kBigThreads) {
+        const float v = __fadd_rn(0.f, __fmul_rn(__ldg(A.scale + i), normal_at(prop_key, (uint32_t)i)));
+        d[i] = v;
+        sq[0] = __fmaf_rn(v, v, sq[0]);
+      }
+      block_sum<1>(sq, red);
+      const float nrm = sqrtf(sq[0]);
+      for (int i = tid; i < D; i += kBigThreads) d[i] = __fdiv_rn(d[i], nrm);
+    }
+    const Key slice_key = fold_in(rng(), 1u);
+    const float level = __fadd_rn(logp_x, logf(uniform01(fold_in(slice_key, 0u))));
+    SliceMachine m;
+    m.start(slice_key, P.eps_dev ? P.eps_dev[c] : P.eps, A);
+    while (m.phase != SliceMachine::DONE) {
+      for (int i = tid; i < D; i += kBigThreads) p[i] = __fadd_rn(x[i], __fmul_rn(m.x, d[i]));
+      __syncthreads();
+      const float lp = big_value_and_grad<TK>(P, p, g, red);
+      __syncthreads();
+      ++evals;
+      m.feed(lp >= level, lp);
+    }
+    if (!loop) {
+      if (tid == 0) {
+        if (A.info.is_accepted) A.info.is_accepted[c] = m.found;
+        if (A.info.num_expansions) A.info.num_expansions[c] = m.num_expansions;
+        if (A.info.num_shrink) A.info.num_shrink[c] = m.n;
+        if (A.info.bracket_left) A.info.bracket_left[c] = m.l;
+        if (A.info.bracket_right) A.info.bracket_right[c] = m.r;
+      }
+    } else if (tid == 0) {
+      if (A.expansions_history) A.expansions_history[(size_t)t * P.C + c] = m.num_expansions;
+      if (A.shrink_history) A.shrink_history[(size_t)t * P.C + c] = m.n;
+    }
+    if (m.found) {  // each thread rewrites the elements it reads
+      for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = __fadd_rn(x[i], __fmul_rn(m.t, d[i]));
+      logp_x = m.lp_t;
+      x = q_out + ro;
+    } else if (q_out != q_in) {  // an out-of-place call carries the old state over
+      for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = x[i];
+    }
+    if (loop && BJX_KEEPS_HISTORY(A.loop, t)) {
+      float* hrow = BJX_HISTORY_ROW(A.loop, t, P.C, c, D);
+      for (int i = tid; i < D; i += kBigThreads) hrow[i] = x[i];
+    }
+  }
+  if (tid == 0) {
+    logp_out[c] = logp_x;
+    if (A.evaluations) atomicAdd(A.evaluations, evals);
+  }
+}
+
 // ---- launch table shared by libbjx (built-in targets) and big-row plug-ins (TK = BJX_TARGET_USER) -------------------------
-enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3, BK_ESS = 4 };
+enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3, BK_ESS = 4, BK_SLICE = 5 };
 struct BigLaunchArgs {
   BigParams P;
   const uint32_t* keys;
@@ -561,6 +640,7 @@ struct BigLaunchArgs {
   InfoPtrs info;
   LangevinArgs langevin;             // BK_LANGEVIN
   EssArgs ess;                       // BK_ESS: q_in, logp_in (logL), q_out, logp_out
+  SliceArgs slice;                   // BK_SLICE: q_in, logp_in, q_out, logp_out
   cudaStream_t stream;
 };
 
@@ -596,6 +676,8 @@ static int big_launch(int kernel_id, const BigLaunchArgs& a) {
                 a.g_out, a.langevin);
     case BK_ESS:
       return go(k_big_ess<TK>, 2, a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.ess);
+    case BK_SLICE:
+      return go(k_big_slice<TK>, 2, a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.slice);
     default:
       return (int)cudaErrorInvalidValue;
   }

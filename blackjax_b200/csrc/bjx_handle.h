@@ -70,6 +70,12 @@ struct bjx_handle_s {
   size_t ess_prior_cap = 0;
   float* ess_ws = nullptr;             // nu [C, D] of the big rows
   size_t ess_ws_cap = 0;
+  // slice sampling's direction scale (bjx_slice.cu): kind -1 until set; [D] or [D, D]
+  int slice_kind = -1;
+  float* slice_scale = nullptr;
+  size_t slice_scale_cap = 0;
+  float* slice_ws = nullptr;           // the direction [C, D] of the big rows
+  size_t slice_ws_cap = 0;
   std::string err;
 };
 

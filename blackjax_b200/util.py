@@ -244,6 +244,34 @@ def sample_elliptical_slice_native(rng_key, state, loglikelihood_fn, mean, cov, 
     return EllipSliceState(q, logl), hist, subiter
 
 
+def sample_slice_sampling_native(rng_key, state, logdensity_fn, num_steps, *, scale=1.0, width=1.0, interval=None,
+                                 max_expansions=10, max_shrinkage=100, thin=1, keep_history=True, chain_offset=0,
+                                 evaluations=None):
+    """``run_inference_algorithm`` for slice sampling without a Python-level loop (libbjx ``bjx_slice_sample``): the
+    same draws as ``num_steps`` calls of ``slice_sampling(logdensity_fn, proposal_generator=direction_proposal(scale),
+    width=width, interval=interval, ...)`` with the step keys ``split(rng_key, T)[t]``.  ``interval`` is ``doubling``
+    (the default) or ``stepping_out`` of :mod:`blackjax_b200.mcmc.slice`; ``width`` a scalar or [C].  ``evaluations``
+    (optional) is a uint64 [1] CUDA tensor to which the call adds the target evaluations it made.  Returns (final
+    SliceState, positions [num_steps // thin, C, D] or None, num_expansions int32 [num_steps, C], num_shrink int32
+    [num_steps, C])."""
+    from ._engine import get_engine
+    from ._lib import check, lib, ptr
+    from .mcmc.slice import SliceState, _check_caps, _interval_code
+    code = _interval_code(interval)
+    _check_caps(max_expansions, max_shrinkage)
+    q, logp = (t.clone() for t in state)
+    eng = get_engine(q, logdensity_fn)
+    eng.ensure_slice_scale(scale)
+    key, hist, n_exp, n_shrink = _native_run("slice_sampling", rng_key, eng, q, num_steps, thin, keep_history,
+                                             chain_offset, torch.int32, torch.int32)
+    w, w_dev = eng._eps(width, "width")
+    check(lib().bjx_slice_sample(eng.h, ptr(key), ptr(q), ptr(logp), int(num_steps), w, ptr(w_dev), code,
+                                 int(max_expansions), int(max_shrinkage), ptr(hist), int(thin), ptr(n_exp),
+                                 ptr(n_shrink), ptr(evaluations)), eng.h)
+    eng._width_keepalive = w_dev  # the launches are asynchronous
+    return SliceState(q, logp), hist, n_exp, n_shrink
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

@@ -519,6 +519,59 @@ int bjx_elliptical_slice_step(bjx_handle_t h, const uint32_t* keys, const float*
 int bjx_elliptical_slice_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logl, int32_t num_steps,
                                 int32_t max_subiter, float* history, int32_t thin, int32_t* subiter_history);
 
+/* ---- Slice sampling (blackjax/mcmc/slice.py: the multivariate slice sampler, blackjax.slice_sampling) ---------------
+ * State (q [C,D], logp [C]) with logp the log-density of the handle's target; initialise it with bjx_init_state (and
+ * discard the gradient row it also writes).  One transition of one chain, all in float32: (prop_key, slice_key) =
+ * split(key); (level_key, interval_key, shrink_key) = split(slice_key, 3); the direction d = n / |n| with n = 0 + scale z
+ * ([D] scale) or scale @ z ([D, D] scale), z = normal(prop_key, (D,)); level = logp + log(uniform(level_key)); t is in
+ * the slice when logp(q + t d) >= level (q + t d unfused; a NaN log-density is never in the slice).
+ *   BJX_SLICE_DOUBLING (Neal's Fig. 4 and Fig. 6): key1, key2 = split(interval_key); L0 = -width uniform(key1),
+ *     R0 = L0 + width; level j widens the left end when uniform(key2, (max_expansions + 1,))[j] < 0.5, else the right
+ *     one, by width 2^j; the bracket is the first level whose ends are both out of the slice, else the last, and
+ *     num_expansions is its index.  A candidate must also pass the acceptance test on that bracket.
+ *   BJX_SLICE_STEPPING_OUT (Fig. 3): u_key, jk_key = split(interval_key); left = -width uniform(u_key),
+ *     right = left + width; j = floor(max_expansions uniform(jk_key)), k = max_expansions - 1 - j; the ends step out by
+ *     width while in the slice, at most j and k times; num_expansions counts the steps.
+ *   Shrinkage (Fig. 5): key = shrink_key; each try takes key, sub = split(key), t = left + uniform(sub) (right - left);
+ *     found = in slice && accepted; then left = t if t < 0, right = t if t >= 0; at most max_shrinkage tries.  A chain
+ *     that finds no point keeps (q, logp) bit for bit and reports is_accepted = 0.
+ * The device evaluates the target fewer times than the reference (the doubling levels one at a time up to the first
+ * whose ends are both out, one point per bisection of the acceptance test, the test only for candidates in the slice)
+ * and decides the same.  The one deviation: the acceptance test stops after max_expansions + 1 bisections and returns
+ * its verdict as it stands; that binds only when width 2^j overflowed to inf, where the reference never stops.
+ * width: a scalar (> 0 and finite) or width_dev [C] per chain (then width is ignored).
+ * Routes (chosen from the handle):
+ *   - every row target and row plug-in, 1 <= dim <= 1024, with a [D] scale, or a [D, D] scale at dim <= 128;
+ *   - every big-row target and big plug-in, 1024 < dim <= 18432 (dim % 4 == 0), with a [D] scale.
+ * BJX_E_UNSUPPORTED: a dense scale beyond 128 dims (from bjx_set_slice_direction_scale), a dense Gaussian target beyond
+ * 128 dims (the tensor-core target path), a plug-in built without the kernels of the row size, and a step or sample
+ * call before bjx_set_slice_direction_scale.  BJX_E_INVALID: a bad width, a negative cap or an unknown interval. */
+#define BJX_SLICE_DOUBLING 0
+#define BJX_SLICE_STEPPING_OUT 1
+/* kind: BJX_METRIC_DIAG (scale [D]) or BJX_METRIC_DENSE (scale [D, D], row-major).  A device array, copied into the
+ * handle. */
+int bjx_set_slice_direction_scale(bjx_handle_t h, int32_t kind, const float* scale);
+typedef struct {            /* optional per-transition outputs (NULL => not written) */
+  uint8_t* is_accepted;     /* [C] 1: shrinkage found a point within max_shrinkage tries */
+  int32_t* num_expansions;  /* [C] */
+  int32_t* num_shrink;      /* [C] shrinkage tries */
+  float* bracket_left;      /* [C] the bracket in t (the current point at t = 0) */
+  float* bracket_right;     /* [C] */
+} bjx_slice_info;
+/* One transition; out may alias in (in place).  Keys follow bjx_set_key_mode. */
+int bjx_slice_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, float* q_out,
+                   float* logp_out, float width, const float* width_dev, int32_t interval, int32_t max_expansions,
+                   int32_t max_shrinkage, const bjx_slice_info* info);
+/* run_inference_algorithm (util.py:150-213): step keys = split(rng_key, num_steps) on the device, then num_steps
+ * transitions in place with no host synchronisation, bit-identical to num_steps step calls with those keys (shared step
+ * key mode, bjx_set_key_mode's chain_offset honoured).  history (optional) float32 [num_steps / thin, C, D];
+ * num_expansions_history and num_shrink_history (optional) int32 [num_steps, C]; evaluations (optional) one device
+ * uint64 to which the target evaluations of the call are added. */
+int bjx_slice_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, int32_t num_steps, float width,
+                     const float* width_dev, int32_t interval, int32_t max_expansions, int32_t max_shrinkage,
+                     float* history, int32_t thin, int32_t* num_expansions_history, int32_t* num_shrink_history,
+                     uint64_t* evaluations);
+
 /* ---- Adjusted MCLMC tuning: adjusted_mclmc_find_L_and_step_size (blackjax/adaptation/adjusted_mclmc_adaptation.py:26-507)
  * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
  * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_adjusted_mclmc_step (BJX_E_UNSUPPORTED
