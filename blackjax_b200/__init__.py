@@ -8,6 +8,8 @@ chains and executed by hand-written sm_90a CUDA kernels through the C ABI in ``i
 import functools as _functools
 
 from . import diagnostics, random, targets, util  # noqa: F401
+from .diagnostics import effective_sample_size as ess  # noqa: F401
+from .diagnostics import ess_bulk, ess_tail, rhat  # noqa: F401
 from ._lib import BjxError  # noqa: F401
 from .adaptation.window_adaptation import build_schedule, window_adaptation  # noqa: F401
 from .adaptation.low_rank_adaptation import build_growing_window_schedule, window_adaptation_low_rank  # noqa: F401

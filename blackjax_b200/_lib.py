@@ -238,6 +238,10 @@ _SIGNATURES = {
     "bjx_potential_scale_reduction": (C.c_int, [C.c_void_p, _f32p, C.c_int32, _f32p, _f32p]),
     "bjx_ess_scratch_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "bjx_effective_sample_size": (C.c_int, [C.c_void_p, _f32p, C.c_int32, _f32p, _f32p]),
+    "bjx_rank_diagnostics_scratch_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "bjx_rank_normalize": (C.c_int, [C.c_void_p, _f32p, C.c_int32, C.c_int32, _f32p, C.c_void_p, C.c_size_t]),
+    "bjx_rank_diagnostics": (C.c_int, [C.c_void_p, _f32p, C.c_int32, C.c_double, _f32p, _f32p, _f32p, C.c_void_p,
+                                       C.c_size_t]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

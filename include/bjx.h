@@ -847,6 +847,23 @@ int bjx_potential_scale_reduction(bjx_handle_t h, const float* history, int32_t 
 int64_t bjx_ess_scratch_floats(int32_t num_samples, int32_t n_chains, int32_t dim);
 int bjx_effective_sample_size(bjx_handle_t h, const float* history, int32_t num_samples, float* ess_out, float* scratch);
 
+/* Rank-normalised split diagnostics (blackjax/diagnostics.py:92-155, 341-522; Vehtari et al. 2021) over the same history
+ * layout.  Each chain is split into halves of h = num_samples / 2 draws (an odd last draw is dropped), giving 2C chains;
+ * every dimension's n = 2C * h pooled draws are ranked with ties broken by pooled index (-0 == +0, NaN after +inf) and
+ * scored z = Phi^-1((r - 3/8) / (n + 1/4)) in float64.  Dimensions are processed dims_per_pass at a time: the calls take
+ * the largest pass width whose scratch fits scratch_bytes (a multiple of 32 when that leaves at least 32).
+ * Rejected with BJX_E_INVALID: num_samples < 4, n >= 2^31, a scratch buffer too small for one dimension per pass, a
+ * scratch pointer not 256-byte aligned.  No host synchronisation. */
+int64_t bjx_rank_diagnostics_scratch_bytes(int32_t num_samples, int32_t n_chains, int32_t dim, int32_t dims_per_pass);
+/* out float32 [h, 2C, D]: the rank-normalised split draws, or with folded != 0 those of |x - median| */
+int bjx_rank_normalize(bjx_handle_t h, const float* history, int32_t num_samples, int32_t folded, float* out,
+                       void* scratch, size_t scratch_bytes);
+/* rhat_out = max(R-hat of the scores, R-hat of the folded scores), ess_bulk_out = ESS of the scores, ess_tail_out =
+ * min(ESS of 1[x <= q_lo], ESS of 1[x >= q_hi]) with q_lo, q_hi the pooled linear quantiles at (1 -+ prob) / 2; each
+ * float32 [D], NULL skips its work.  A column with a NaN draw reports NaN in all three.  prob in (0, 1). */
+int bjx_rank_diagnostics(bjx_handle_t h, const float* history, int32_t num_samples, double prob, float* rhat_out,
+                         float* ess_bulk_out, float* ess_tail_out, void* scratch, size_t scratch_bytes);
+
 #ifdef __cplusplus
 }
 #endif
