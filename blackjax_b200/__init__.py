@@ -30,8 +30,10 @@ from .util import run_inference_algorithm, sample_hmc_native, sample_mclmc_nativ
 from .util import sample_adjusted_mclmc_native, sample_gist_native  # noqa: F401
 from .util import sample_barker_native, sample_mala_native  # noqa: F401
 from .util import sample_elliptical_slice_native, sample_slice_sampling_native  # noqa: F401
+from .util import sample_random_walk_native  # noqa: F401
 from .mcmc import elliptical_slice as _elliptical_slice
 from .mcmc import slice as _slice
+from .mcmc import random_walk as _random_walk
 from .mcmc import barker as _barker
 from .mcmc import mala as _mala
 from .mcmc.composed import step_size as _gist_step_size
@@ -69,5 +71,10 @@ barker_proposal = barker  # blackjax/__init__.py:141
 elliptical_slice = GenerateSamplingAPI(_elliptical_slice.as_top_level_api, _elliptical_slice.init,  # blackjax/__init__.py:134
                                        _elliptical_slice.build_kernel)
 slice_sampling = GenerateSamplingAPI(_slice.as_top_level_api, _slice.init, _slice.build_kernel)  # blackjax/__init__.py:134
+rmh = GenerateSamplingAPI(_random_walk.rmh_as_top_level_api, _random_walk.init, _random_walk.build_rmh)  # :113
+irmh = GenerateSamplingAPI(_random_walk.irmh_as_top_level_api, _random_walk.init, _random_walk.build_irmh)  # :114-116
+additive_step_random_walk = GenerateSamplingAPI(_random_walk.additive_step_random_walk, _random_walk.init,  # :125-129
+                                                _random_walk.build_additive_step)
+additive_step_random_walk.register_factory("normal_random_walk", _random_walk.normal_random_walk)
 
 __version__ = "0.1.0"

@@ -430,6 +430,49 @@ class Engine:
         self._width_keepalive = w_dev  # the launch is asynchronous
         return qo, lo
 
+    def ensure_rw_proposal(self, kind, sigma, mean=None):
+        """Install random-walk Metropolis's Gaussian proposal (libbjx ``bjx_set_rw_proposal``) unless this exact content
+        is installed, keyed as ``ensure_slice_scale``: ``kind`` ``RW_ADDITIVE`` (y = x + lin) or ``RW_INDEPENDENT``
+        (y = mean + lin, ``mean`` a scalar or [D]); ``sigma`` a scalar (expanded to [D]), [D] or [D, D]."""
+        def content_key(t):
+            if t is None:
+                return ("none",)
+            if isinstance(t, torch.Tensor):
+                return (t.data_ptr(), tuple(t.shape), t._version, str(t.device))
+            return ("scalar", float(t)) if np.ndim(t) == 0 else None
+        key = (int(kind), content_key(sigma), content_key(mean))
+        given = (sigma, mean)
+        if None not in key and key == getattr(self, "_rw_key", None):
+            return
+        s = torch.as_tensor(sigma, dtype=torch.float32, device=self.device)
+        if s.ndim == 0:
+            s = s.expand(self.D)
+        if s.ndim == 1 and s.shape[0] == self.D:
+            sigma_kind = _lib.METRIC_DIAG
+        elif s.ndim == 2 and tuple(s.shape) == (self.D, self.D):
+            sigma_kind = _lib.METRIC_DENSE
+        else:
+            raise ValueError(f"sigma has shape {tuple(s.shape)}, expected (), ({self.D},) or ({self.D}, {self.D})")
+        s = s.contiguous()
+        m = None
+        if kind == _lib.RW_INDEPENDENT:
+            m = torch.broadcast_to(torch.as_tensor(mean, dtype=torch.float32, device=self.device), (self.D,)).contiguous()
+        check(lib().bjx_set_rw_proposal(self.h, int(kind), ptr(m), sigma_kind, ptr(s)), self.h)
+        self._rw = (given, s, m)  # the key's tensors stay alive, so their addresses are not reused
+        self._rw_key = key if None not in key else None
+
+    def rw_step(self, keys, q, logp, correct=False, out=None, info_fields=None, chain_offset=0):
+        """One random-walk Metropolis transition (libbjx ``bjx_rw_step``) with the installed proposal."""
+        keys = as_keys(keys, self.C, self.device)
+        self._key_mode(keys, chain_offset)
+        q = _f32(q, (self.C, self.D), "position")
+        logp = _f32(logp, (self.C,), "logdensity")
+        qo, lo = out if out is not None else (torch.empty_like(q), torch.empty_like(logp))
+        info = self._info(info_fields or {}, _lib.RwInfo)
+        check(lib().bjx_rw_step(self.h, ptr(keys), ptr(q), ptr(logp), ptr(qo), ptr(lo), int(bool(correct)),
+                                C.byref(info)), self.h)
+        return qo, lo
+
     def adjusted_mclmc_num_steps(self, device_rule, avg, random_generator_arg):
         """The step counts int32 [C] of a dynamic rule ``device_rule = (rule, min_steps)`` at a per-chain ``avg`` [C]
         (libbjx ``bjx_adjusted_mclmc_num_steps``); random_generator_arg [C, 2] is read, not advanced.  The fixed rule

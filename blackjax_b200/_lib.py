@@ -13,6 +13,7 @@ AMCLMC_STEPS_FIXED, AMCLMC_STEPS_RANDINT, AMCLMC_STEPS_UNIFORM = 0, 1, 2
 GIST_TRAJECTORY_LENGTH, GIST_STEP_SIZE = 0, 1
 GIST_SYMMETRIC, GIST_ASYMMETRIC = 0, 1
 SLICE_DOUBLING, SLICE_STEPPING_OUT = 0, 1
+RW_ADDITIVE, RW_INDEPENDENT = 0, 1
 
 _f32p = C.c_void_p  # device pointers travel as integers
 
@@ -64,6 +65,10 @@ class EllipticalSliceInfo(C.Structure):
 class SliceInfo(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("is_accepted", "num_expansions", "num_shrink", "bracket_left",
                                           "bracket_right")]
+
+
+class RwInfo(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("acceptance_rate", "is_accepted")]
 
 
 class LapsBurnInConfig(C.Structure):
@@ -153,6 +158,9 @@ _SIGNATURES = {
                                  C.c_int32, C.POINTER(SliceInfo)]),
     "bjx_slice_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, C.c_int32, C.c_float, _f32p, C.c_int32, C.c_int32,
                                    C.c_int32, _f32p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bjx_set_rw_proposal": (C.c_int, [C.c_void_p, C.c_int32, _f32p, C.c_int32, _f32p]),
+    "bjx_rw_step": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32, C.POINTER(RwInfo)]),
+    "bjx_rw_sample": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, C.c_int32, C.c_int32, _f32p, C.c_int32, _f32p]),
     "bjx_laps_state_floats": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "bjx_laps_init": (C.c_int, [C.c_void_p, _f32p, _f32p, _f32p, _f32p, _f32p, C.c_int32]),
     "bjx_laps_burn_in_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint32), C.c_int32, C.c_int32, _f32p, _f32p, _f32p,

@@ -47,3 +47,8 @@ class GenerateSamplingAPI:
 
     def __call__(self, *args, **kwargs):
         return self.differentiable(*args, **kwargs)
+
+    def register_factory(self, name, callable):
+        """blackjax/__init__.py:79-80: expose ``callable`` as the attribute ``name`` (e.g.
+        ``additive_step_random_walk.normal_random_walk``)."""
+        setattr(self, name, callable)

@@ -191,6 +191,8 @@ extern "C" int bjx_destroy(bjx_handle_t h) {
   if (h->ess_ws) cudaFree(h->ess_ws);
   if (h->slice_scale) cudaFree(h->slice_scale);
   if (h->slice_ws) cudaFree(h->slice_ws);
+  if (h->rw_sigma) cudaFree(h->rw_sigma);
+  if (h->rw_mean) cudaFree(h->rw_mean);
   if (h->h_flag) cudaFreeHost(h->h_flag);
   delete h;
   return 0;
@@ -417,16 +419,18 @@ int dispatch(bjx_handle_t h, int kernel_id, bool target_dependent, LaunchArgs& a
   const bool langevin = kernel_id == K_LANGEVIN || kernel_id == K_LANGEVIN_CHAINS;
   const bool ess = kernel_id == K_ESS || kernel_id == K_ESS_CHAINS;
   const bool slice = kernel_id == K_SLICE || kernel_id == K_SLICE_CHAINS;
-  // MALA, Barker, elliptical slice and slice sampling integrate nothing
-  a.general_integrator = h->general_integrator && !langevin && !ess && !slice;
-  // elliptical slice and slice sampling have no metric: their dense variants are the small dense prior's and the small
-  // dense direction scale's
+  const bool rw = kernel_id == K_RW || kernel_id == K_RW_CHAINS;
+  // MALA, Barker, elliptical slice, slice sampling and random-walk Metropolis integrate nothing
+  a.general_integrator = h->general_integrator && !langevin && !ess && !slice && !rw;
+  // elliptical slice, slice sampling and random-walk Metropolis have no metric: their dense variants are the small dense
+  // prior's, the small dense direction scale's and the small dense sigma's
   const bool dm = ess ? a.ess.prior == ESS_PRIOR_DENSE
                       : slice ? h->slice_kind == BJX_METRIC_DENSE
+                      : rw ? h->rw_sigma_kind == BJX_METRIC_DENSE
                       : (h->metric_small_dense || h->metric_kind == BJX_METRIC_LOW_RANK) &&
                             !(langevin && a.langevin.kind == LANGEVIN_MALA);  // MALA has no metric
   if (kernel_id == K_NUTS_CHAINS || kernel_id == K_GIST_CHAINS || kernel_id == K_ESS_CHAINS ||
-      kernel_id == K_SLICE_CHAINS)  // the persistent grids
+      kernel_id == K_SLICE_CHAINS || kernel_id == K_RW_CHAINS)  // the persistent grids
     BJX_CUDA(cudaMemsetAsync(h->chain_queue, 0, sizeof(int), h->stream));
   int rc;
   const int tk = target_dependent ? h->cfg.target.kind : (int)BJX_TARGET_FUNNEL;

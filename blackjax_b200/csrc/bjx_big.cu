@@ -400,3 +400,13 @@ int bjx_big_slice(bjx_handle_t h, const uint32_t* keys, const float* q_in, const
   a.slice = A;
   return big_dispatch(h, BK_SLICE, a);
 }
+// Random-walk Metropolis on the big rows: one transition (A.loop.step_keys == nullptr) or the native loop (bjx_rw.cu)
+int bjx_big_rw(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, float* q_out,
+               float* logp_out, const RwArgs& A) {
+  BigLaunchArgs a{};
+  a.P = big_params(h, 0.f, nullptr);
+  a.keys = keys; a.q_in = q_in; a.logp_in = logp_in;
+  a.q_out = q_out; a.logp_out = logp_out;
+  a.rw = A;
+  return big_dispatch(h, BK_RW, a);
+}

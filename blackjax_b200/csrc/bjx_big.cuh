@@ -628,8 +628,74 @@ __global__ void __launch_bounds__(kBigThreads) k_big_slice(BigParams P, const ui
   }
 }
 
+// Random-walk Metropolis transitions (the warp kernels' rw_transition_row, bjx_kernels.cuh) with a [D] sigma.  The
+// proposal y and its gradient scratch, which the target addresses freely, sit in shared memory; x is re-read from its
+// row, each thread using the elements t + 768 k that it also writes on acceptance.  One launch runs one transition
+// (A.loop.step_keys == nullptr: keys and A.info as bjx_rw_step's) or the A.loop.num_steps transitions of the native loop
+// in place.
+template <int TK>
+__global__ void __launch_bounds__(kBigThreads) k_big_rw(BigParams P, const uint32_t* __restrict__ keys, const float* q_in,
+                                                        const float* logp_in, float* q_out, float* logp_out, RwArgs A) {
+  extern __shared__ __align__(16) float sm[];
+  float *y = sm, *g = sm + P.D, *red = sm + 2 * (size_t)P.D;
+  const int c = blockIdx.x, D = P.D, tid = threadIdx.x;
+  const size_t ro = (size_t)c * D;
+  const bool loop = A.loop.step_keys != nullptr;
+  const int T = loop ? A.loop.num_steps : 1;
+  const bool independent = A.kind == RW_INDEPENDENT, correct = A.correct != 0;
+  const float* x = q_in + ro;  // the native loop: q_in == q_out, rewritten on acceptance
+  float logp_x = logp_in[c];
+  for (int t = 0; t < T; ++t) {
+    auto rng = [&]() {
+      const uint32_t* kt = loop ? A.loop.step_keys + 2 * t : keys;
+      return P.key_shared ? fold_in(Key{kt[0], kt[1]}, P.chain_offset + (uint32_t)c) : Key{kt[2 * c], kt[2 * c + 1]};
+    };
+    {
+      const Key key_proposal = fold_in(rng(), 0u);
+      for (int i = tid; i < D; i += kBigThreads) {
+        const float lin = __fmul_rn(__ldg(A.sigma + i), normal_at(key_proposal, (uint32_t)i));
+        y[i] = __fadd_rn(independent ? __ldg(A.mean + i) : x[i], lin);
+      }
+    }
+    __syncthreads();
+    const float logp_y = big_value_and_grad<TK>(P, y, g, red);
+    __syncthreads();
+    float sq[2] = {0.f, 0.f};  // sq_x, sq_y
+    if (correct) {
+      for (int i = tid; i < D; i += kBigThreads) {
+        const float m = __ldg(A.mean + i), is = __ldg(A.inv_sigma + i);
+        sq[0] = __fadd_rn(sq[0], rw_q_term(x[i], m, is));
+        sq[1] = __fadd_rn(sq[1], rw_q_term(y[i], m, is));
+      }
+      block_sum<2>(sq, red);
+    }
+    const float p_acc = clip_max1(expf(rw_log_accept(logp_x, logp_y, correct, sq[0], sq[1])));
+    const bool acc = uniform01(fold_in(rng(), 1u)) < p_acc;
+    if (tid == 0) {
+      if (!loop) {
+        if (A.info.acceptance_rate) A.info.acceptance_rate[c] = p_acc;
+        if (A.info.is_accepted) A.info.is_accepted[c] = acc;
+      } else if (A.acceptance_history) {
+        A.acceptance_history[(size_t)t * P.C + c] = p_acc;
+      }
+    }
+    if (acc) {  // each thread rewrites the elements it reads
+      for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = y[i];
+      logp_x = logp_y;
+      x = q_out + ro;
+    } else if (q_out != q_in) {  // an out-of-place call carries the old state over
+      for (int i = tid; i < D; i += kBigThreads) q_out[ro + i] = x[i];
+    }
+    if (loop && BJX_KEEPS_HISTORY(A.loop, t)) {
+      float* hrow = BJX_HISTORY_ROW(A.loop, t, P.C, c, D);
+      for (int i = tid; i < D; i += kBigThreads) hrow[i] = x[i];
+    }
+  }
+  if (tid == 0) logp_out[c] = logp_x;
+}
+
 // ---- launch table shared by libbjx (built-in targets) and big-row plug-ins (TK = BJX_TARGET_USER) -------------------------
-enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3, BK_ESS = 4, BK_SLICE = 5 };
+enum BigKernelId { BK_INIT = 0, BK_LEAPFROG = 1, BK_HMC = 2, BK_LANGEVIN = 3, BK_ESS = 4, BK_SLICE = 5, BK_RW = 6 };
 struct BigLaunchArgs {
   BigParams P;
   const uint32_t* keys;
@@ -641,6 +707,7 @@ struct BigLaunchArgs {
   LangevinArgs langevin;             // BK_LANGEVIN
   EssArgs ess;                       // BK_ESS: q_in, logp_in (logL), q_out, logp_out
   SliceArgs slice;                   // BK_SLICE: q_in, logp_in, q_out, logp_out
+  RwArgs rw;                         // BK_RW: q_in, logp_in, q_out, logp_out
   cudaStream_t stream;
 };
 
@@ -678,6 +745,8 @@ static int big_launch(int kernel_id, const BigLaunchArgs& a) {
       return go(k_big_ess<TK>, 2, a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.ess);
     case BK_SLICE:
       return go(k_big_slice<TK>, 2, a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.slice);
+    case BK_RW:
+      return go(k_big_rw<TK>, 2, a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out, a.rw);
     default:
       return (int)cudaErrorInvalidValue;
   }

@@ -76,12 +76,24 @@ struct bjx_handle_s {
   size_t slice_scale_cap = 0;
   float* slice_ws = nullptr;           // the direction [C, D] of the big rows
   size_t slice_ws_cap = 0;
+  // random-walk Metropolis's Gaussian proposal (bjx_rw.cu): kind -1 until set; sigma [D] or [D, D]; mean [D] and
+  // 1 / sigma [D] (a [D] sigma)
+  int rw_kind = -1;
+  int rw_sigma_kind = -1;
+  float* rw_sigma = nullptr;
+  size_t rw_sigma_cap = 0;
+  float* rw_mean = nullptr;      // mean [D] | 1 / sigma [D]
+  size_t rw_mean_cap = 0;
   std::string err;
 };
 
 int bjx_fail(bjx_handle_t h, int code, const std::string& msg);
 int bjx_ensure_nuts_ws(bjx_handle_t h);  // the NUTS workspace of bjx_api.cu (shared with the dense path)
 int bjx_cuda_fail(bjx_handle_t h, cudaError_t e, const char* where);
+// The [D] (kind BJX_METRIC_DIAG) or [D, D] (BJX_METRIC_DENSE, dim <= 128) float32 device array src copied into the
+// handle's grow-only buffer dst on its stream (bjx_slice.cu): slice sampling's direction scale, random-walk Metropolis's
+// sigma.  A refusal names the array `what`.
+int bjx_store_scale(bjx_handle_t h, int32_t kind, const float* src, float*& dst, size_t& cap, const char* what);
 
 // Grow-only device buffer: *buf holds at least `need` units (elements or bytes, as *cap counts them) afterwards.
 template <class T>

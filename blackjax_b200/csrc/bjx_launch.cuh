@@ -12,7 +12,7 @@ namespace bjx {
 enum SizeClass { SC_V1 = 0, SC_V2, SC_V4, SC_V8, SC_S1, SC_S4, SC_BIG, SC_NONE };  // SC_BIG: CTA-per-chain (bjx_big.cu)
 enum KernelId { K_INIT = 0, K_MOMENTUM, K_LEAPFROG, K_ENERGY, K_TURNING, K_HMC, K_NUTS_INIT, K_NUTS_DOUBLING, K_MHMC, K_GHMC, K_NUTS_CHAINS,
                K_MCLMC, K_AMCLMC, K_MCLMC_TUNE, K_AMCLMC_TUNE, K_LAPS_BURN_IN, K_GIST, K_GIST_CHAINS, K_LANGEVIN,
-               K_LANGEVIN_CHAINS, K_ESS, K_ESS_CHAINS, K_SLICE, K_SLICE_CHAINS };
+               K_LANGEVIN_CHAINS, K_ESS, K_ESS_CHAINS, K_SLICE, K_SLICE_CHAINS, K_RW, K_RW_CHAINS };
 
 struct LaunchArgs {
   Params P;
@@ -29,6 +29,7 @@ struct LaunchArgs {
   LangevinArgs langevin;
   EssArgs ess;         // K_ESS / K_ESS_CHAINS: q_in, logp_in (logL), q_out, logp_out
   SliceArgs slice;     // K_SLICE / K_SLICE_CHAINS: q_in, logp_in, q_out, logp_out
+  RwArgs rw;           // K_RW / K_RW_CHAINS: q_in, logp_in, q_out, logp_out
   const uint32_t* keys;
   const float *q_in, *logp_in, *g_in;
   float *q_out, *logp_out, *g_out;
@@ -88,7 +89,7 @@ static void allow_dynamic_smem(K kern, size_t bytes) {
   if (bytes > 48 * 1024 - 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 }
 
-// A persistent grid over the chains (k_nuts_chains, k_gist_chains, k_ess_chains, k_slice_chains), whose warps take the chains from the
+// A persistent grid over the chains (k_nuts_chains, k_gist_chains, k_ess_chains, k_slice_chains, k_rw_chains), whose warps take the chains from the
 // queue dispatch() zeroed: every CTA that stays resident (registers, shared memory) on each SM, at most one per
 // kWarpsPerBlock chains.
 template <class K, class... Args>
@@ -138,6 +139,18 @@ static int launch_slice(int kernel_id, const LaunchArgs& a, dim3 grid) {
     return 0;
   }
   launch_persistent(k_slice_chains<R, TK, DM>, a, smem, a.P, a.q_out, a.logp_out, a.slice);
+  return 0;
+}
+
+// Random-walk Metropolis: shared memory only for the target's and the dense sigma's row slices
+template <class R, int TK, bool DM>
+static int launch_rw(int kernel_id, const LaunchArgs& a, dim3 grid, size_t smem) {
+  if (kernel_id == K_RW) {
+    k_rw_transition<R, TK, DM><<<grid, kThreads, smem, a.stream>>>(a.P, a.keys, a.q_in, a.logp_in, a.q_out, a.logp_out,
+                                                                     a.rw);
+    return 0;
+  }
+  launch_persistent(k_rw_chains<R, TK, DM>, a, smem, a.P, a.q_out, a.logp_out, a.rw);
   return 0;
 }
 
@@ -241,6 +254,11 @@ static int launch_gen(int kernel_id, const LaunchArgs& a) {
     case K_SLICE_CHAINS:
       // velocity Verlet instances only (nothing is integrated); dm selects the small dense direction scale (dim <= 128)
       if constexpr (!GEN && (!DM || R::NS <= 4)) return launch_slice<R, TK, DM>(kernel_id, a, grid);
+      break;
+    case K_RW:
+    case K_RW_CHAINS:
+      // velocity Verlet instances only (nothing is integrated); dm selects the small dense sigma (dim <= 128)
+      if constexpr (!GEN && (!DM || R::NS <= 4)) return launch_rw<R, TK, DM>(kernel_id, a, grid, smem);
       break;
     case K_NUTS_CHAINS:  // the row and the checkpoints of every doubling in shared memory
       launch_persistent(k_nuts_chains<R, TK, DM, GEN>, a,

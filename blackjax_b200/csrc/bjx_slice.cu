@@ -17,22 +17,28 @@ using namespace bjx;
 int bjx_big_slice(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, float* q_out,
                   float* logp_out, float width, const float* width_dev, const SliceArgs& A);
 
-extern "C" int bjx_set_slice_direction_scale(bjx_handle_t h, int32_t kind, const float* scale) {
-  if (!h || !scale) return bjx_fail(h, BJX_E_INVALID, "null argument");
-  BJX_CUDA(cudaSetDevice(h->cfg.device));
+int bjx_store_scale(bjx_handle_t h, int32_t kind, const float* src, float*& dst, size_t& cap, const char* what) {
   const int D = h->cfg.dim;
   size_t elems;
   if (kind == BJX_METRIC_DIAG) {
     elems = D;
   } else if (kind == BJX_METRIC_DENSE) {
-    if (D > 128) return bjx_fail(h, BJX_E_UNSUPPORTED, "a dense slice direction scale is built for dim <= 128");
+    if (D > 128) return bjx_fail(h, BJX_E_UNSUPPORTED, std::string("a dense ") + what + " is built for dim <= 128");
     elems = (size_t)D * D;
   } else {
-    return bjx_fail(h, BJX_E_INVALID, "the direction scale has the wrong number of dimensions: expected 1 or 2");
+    return bjx_fail(h, BJX_E_INVALID, std::string("the ") + what + " has the wrong number of dimensions: expected 1 or 2");
   }
-  int rc = bjx_grow(h, h->slice_scale, h->slice_scale_cap, elems, sizeof(float));
+  int rc = bjx_grow(h, dst, cap, elems, sizeof(float));
   if (rc) return rc;
-  BJX_CUDA(cudaMemcpyAsync(h->slice_scale, scale, elems * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  BJX_CUDA(cudaMemcpyAsync(dst, src, elems * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  return 0;
+}
+
+extern "C" int bjx_set_slice_direction_scale(bjx_handle_t h, int32_t kind, const float* scale) {
+  if (!h || !scale) return bjx_fail(h, BJX_E_INVALID, "null argument");
+  BJX_CUDA(cudaSetDevice(h->cfg.device));
+  int rc = bjx_store_scale(h, kind, scale, h->slice_scale, h->slice_scale_cap, "slice direction scale");
+  if (rc) return rc;
   h->slice_kind = kind;
   return 0;
 }

@@ -4,3 +4,4 @@ from . import composed  # noqa: F401,E402
 from . import barker, mala  # noqa: F401,E402
 from . import elliptical_slice  # noqa: F401,E402
 from . import slice  # noqa: F401,E402
+from . import random_walk  # noqa: F401,E402

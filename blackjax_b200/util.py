@@ -272,6 +272,28 @@ def sample_slice_sampling_native(rng_key, state, logdensity_fn, num_steps, *, sc
     return SliceState(q, logp), hist, n_exp, n_shrink
 
 
+def sample_random_walk_native(rng_key, state, logdensity_fn, num_steps, *, proposal, proposal_logdensity_fn=None,
+                              thin=1, keep_history=True, chain_offset=0):
+    """``run_inference_algorithm`` for random-walk Metropolis without a Python-level loop (libbjx ``bjx_rw_sample``):
+    the same draws as ``num_steps`` step calls with the step keys ``split(rng_key, T)[t]``.  ``proposal`` is a
+    descriptor of :mod:`blackjax_b200.mcmc.random_walk` (``normal``, ``gaussian_proposal`` or
+    ``gaussian_distribution``) and ``proposal_logdensity_fn`` None or its ``gaussian_logdensity``.  Returns (final
+    RWState, positions [num_steps // thin, C, D] or None, acceptance rates [num_steps, C])."""
+    from ._engine import get_engine
+    from ._lib import check, lib, ptr
+    from .mcmc.random_walk import RWState, _correct_of, _proposal_of
+    kind, sigma, mean = _proposal_of(proposal, getattr(proposal, "rw_role", "proposal"))
+    correct = _correct_of((kind, sigma, mean), proposal_logdensity_fn)
+    q, logp = (t.clone() for t in state)
+    eng = get_engine(q, logdensity_fn)
+    eng.ensure_rw_proposal(kind, sigma, mean)
+    key, hist, acc = _native_run("random_walk", rng_key, eng, q, num_steps, thin, keep_history, chain_offset,
+                                 torch.float32)
+    check(lib().bjx_rw_sample(eng.h, ptr(key), ptr(q), ptr(logp), int(num_steps), int(correct), ptr(hist), int(thin),
+                              ptr(acc)), eng.h)
+    return RWState(q, logp), hist, acc
+
+
 def run_inference_algorithm(rng_key, inference_algorithm, num_steps, initial_state=None, initial_position=None,
                             transform=lambda state, info: (state, info), collect=True):
     """``keys = split(rng_key, num_steps)`` then ``num_steps`` calls of ``step`` (util.py:200-211).

@@ -572,6 +572,40 @@ int bjx_slice_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* l
                      float* history, int32_t thin, int32_t* num_expansions_history, int32_t* num_shrink_history,
                      uint64_t* evaluations);
 
+/* ---- Random-walk Metropolis (blackjax/mcmc/random_walk.py: blackjax.additive_step_random_walk, rmh, irmh) -----------
+ * State (q [C,D], logp [C]) with logp the log-density of the handle's target; initialise it with bjx_init_state (and
+ * discard the gradient row it also writes).  The stored logp is used as given, never re-evaluated.  One transition of one
+ * chain, all in float32: (key_proposal, key_accept) = split(key); z = normal(key_proposal, (D,)); lin = sigma z ([D]
+ * sigma) or sigma @ z ([D, D] sigma); the proposal is y = q + lin (BJX_RW_ADDITIVE) or y = mean + lin
+ * (BJX_RW_INDEPENDENT); with E(a, b) = -logp(b) - f(b, a), log_p_accept = E(y, x) - E(x, y) (NaN -> -inf),
+ * acceptance_rate = min(1, exp(log_p_accept)) and the proposal is accepted when uniform(key_accept) < acceptance_rate.
+ * f = 0 unless correct != 0; then f(b, a) = -0.5 sum ((a - mean) / sigma)^2, the log-density of the independent proposal
+ * N(mean, diag(sigma)^2) at a without its constant terms (they cancel).  A rejected chain keeps (q, logp) bit for bit.
+ * Routes (chosen from the handle):
+ *   - every row target and row plug-in, 1 <= dim <= 1024, with a [D] sigma, or a [D, D] sigma at dim <= 128;
+ *   - every big-row target and big plug-in, 1024 < dim <= 18432 (dim % 4 == 0), with a [D] sigma.
+ * BJX_E_UNSUPPORTED: a dense sigma beyond 128 dims (from bjx_set_rw_proposal), a dense Gaussian target beyond 128 dims
+ * (the tensor-core target path), a plug-in built without the kernels of the row size, a step or sample call before
+ * bjx_set_rw_proposal, and correct != 0 with a dense sigma or an additive proposal. */
+#define BJX_RW_ADDITIVE 0
+#define BJX_RW_INDEPENDENT 1
+/* kind: BJX_RW_ADDITIVE (mean NULL) or BJX_RW_INDEPENDENT (mean [D]); sigma_kind: BJX_METRIC_DIAG (sigma [D]) or
+ * BJX_METRIC_DENSE (sigma [D, D], row-major, dim <= 128).  Device arrays, copied into the handle. */
+int bjx_set_rw_proposal(bjx_handle_t h, int32_t kind, const float* mean, int32_t sigma_kind, const float* sigma);
+typedef struct {            /* optional per-transition outputs (NULL => not written) */
+  float* acceptance_rate;   /* [C] */
+  uint8_t* is_accepted;     /* [C] */
+} bjx_rw_info;
+/* One transition; out may alias in (in place, both of (q, logp)).  Keys follow bjx_set_key_mode. */
+int bjx_rw_step(bjx_handle_t h, const uint32_t* keys, const float* q_in, const float* logp_in, float* q_out,
+                float* logp_out, int32_t correct, const bjx_rw_info* info);
+/* run_inference_algorithm (util.py:150-213): step keys = split(rng_key, num_steps) on the device, then num_steps
+ * transitions in place with no host synchronisation, bit-identical to num_steps step calls with those keys (shared step
+ * key mode, bjx_set_key_mode's chain_offset honoured).  history (optional) float32 [num_steps / thin, C, D];
+ * acceptance_history (optional) float32 [num_steps, C]. */
+int bjx_rw_sample(bjx_handle_t h, const uint32_t* rng_key, float* q, float* logp, int32_t num_steps, int32_t correct,
+                  float* history, int32_t thin, float* acceptance_history);
+
 /* ---- Adjusted MCLMC tuning: adjusted_mclmc_find_L_and_step_size (blackjax/adaptation/adjusted_mclmc_adaptation.py:26-507)
  * Every chain runs the reference's single-chain tuner with its own key, as jax.vmap over chains would, and ends with its own
  * (L, step_size, inverse_mass_matrix).  Supported configurations are those of bjx_adjusted_mclmc_step (BJX_E_UNSUPPORTED
